@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the north-star path: Router::matches for a batch of PUBLISH topics at 10 M subscriptions.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl own|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl own|reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path (tokenise -> trie walk -> per-topic match lists) over one batch of
 synthetic topics (workload C3 of BASELINE.json: 10 M subscriptions, 30 % '+', 5 % '#', 6-level IoT topics,
@@ -12,7 +12,8 @@ batch of topics of its shard, no collective -> "scaling": "weak"); `multi_gpu` a
 strong-scaling leg (one mixed batch partitioned by a device kernel, matched, gathered), and `parity_check` verifies
 the gathered lists of a 60 K-topic sample against the oracle on rank 0.
 
-Prints ONE JSON line (rank 0).  See DESIGN.md §"Measurement" for every key.
+Prints ONE JSON line (rank 0).  See DESIGN.md §"Measurement" for every key.  --dump-outputs DIR writes the match lists of
+the last timed step to DIR as .npy files (see _dump_outputs), so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -47,17 +48,13 @@ def _args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--e2e-steps", type=int, default=None)
     ap.add_argument("--no-c4", action="store_true", help="skip the retained-tree (config C4) leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (rank 0) to DIR/<name>.npy, float64, at most 64 MB")
     return ap.parse_args()
 
 
 def _peaks():
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        try:
-            return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3 (not a measured figure)"
 
 
 class ClockSampler:
@@ -121,7 +118,7 @@ def _workload_desc(cfg, world):
             f"reg/site/dev/sen/met/ch over R{cfg.R}xS{cfg.S}xD{cfg.D}xK{cfg.K}xM{cfg.M}xF{cfg.F}, "
             f"{cfg.n_topics}-topic uniform batch per GPU, seed {cfg.seed:#x}"
             + (f", subscriptions sharded by topic-root hash over {world} GPUs (root-wildcards replicated)" if world > 1 else "")
-            + "; L2: the device tables (GBs) and the rotated distinct batches are far larger than the 126 MB L2, no flush between steps")
+            + "; L2: the device tables (GBs) and the rotated distinct batches are far larger than the 50 MB L2, no flush between steps")
 
 
 # ======================================================================================================
@@ -170,6 +167,37 @@ def run_reference(args):
         "gpu_launches": 0,
     }
     _emit(line)
+
+
+DUMP_SAMPLE_TOPICS = 65_536
+DUMP_MAX_BYTES = 64_000_000
+
+
+def _dump_outputs(out_dir: Path, spans: np.ndarray, ids: np.ndarray, status: np.ndarray) -> None:
+    """What a caller of gm_match_batch_device receives for one batch, in a form two builds can compare file by file:
+    counts.npy (every topic's match count, -1 for a topic the path rejected; float64), status.npy (every topic's status
+    code; float32) and, in float64, for a fixed seeded sample of topics (sample_topics.npy, ascending), the id multiset
+    of each one, sorted:
+    sample_ids.npy[sample_offsets[i] : sample_offsets[i + 1]] belongs to topic sample_topics[i].  The order of ids inside
+    a list and the placement of the lists in the id buffer depend on scheduling, so the raw buffers are not dumped."""
+    n = len(status)
+    counts = spans[:, 1].astype(np.int64)
+    counts[status != 0] = -1
+    pick = np.sort(np.random.default_rng(0xD0_5EED).choice(n, size=min(n, DUMP_SAMPLE_TOPICS), replace=False))
+    id_budget = (DUMP_MAX_BYTES - 12 * n - 16 * (len(pick) + 1) - 4096) // 8     # counts f64 + status f32 per topic, the rest ids
+    if id_budget <= 0:
+        raise ValueError(f"--dump-outputs: a {n}-topic batch does not fit {DUMP_MAX_BYTES} bytes; use a smaller --topics")
+    c = np.maximum(counts[pick], 0)
+    keep = np.cumsum(c) <= id_budget                      # a prefix of the sample (heavy hitters could overflow the budget)
+    pick, c = pick[keep], c[keep]
+    starts = np.zeros(len(pick) + 1, dtype=np.int64)
+    np.cumsum(c, out=starts[1:])
+    src = np.repeat(spans[pick, 0].astype(np.int64), c) + np.arange(int(starts[-1]), dtype=np.int64) - np.repeat(starts[:-1], c)
+    vals = ids.view(np.uint32)[src]
+    vals = vals[np.lexsort((vals, np.repeat(np.arange(len(pick)), c)))]
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, a in (("counts", counts), ("status", status.astype(np.float32)), ("sample_topics", pick), ("sample_offsets", starts), ("sample_ids", vals)):
+        np.save(out_dir / f"{name}.npy", a if a.dtype == np.float32 else a.astype(np.float64))
 
 
 # ======================================================================================================
@@ -430,6 +458,8 @@ def run_own(args):
     kms = eng.kernel_ms(min(64, args.steps))
     clocks = sampler.stop() if sampler else None
     value = world * n * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:               # the buffers still hold the last timed step; the next leg overwrites them
+        _dump_outputs(Path(args.dump_outputs), d_spans.cpu().numpy(), d_ids[:int(d_needed.item())].cpu().numpy(), d_status.cpu().numpy())
 
     # the same loop in descriptor mode (8 B per matched filter instead of 4 B per matched id): explains the e2e number
     d_desc = torch.empty((int(desc_max * 1.25) + 1024, 2), dtype=torch.int32, device=dev)
@@ -585,7 +615,7 @@ def run_own(args):
             "warmup": max(3, args.warmup), "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "u32", "data": "synthetic",
             "config": {"workload": _workload_desc(cfg, world)},
-            "details": {"l2": f"device tables {st['device_bytes'] / 1e9:.2f} GB >> 126 MB L2; {B} distinct topic batches rotated",
+            "details": {"l2": f"device tables {st['device_bytes'] / 1e9:.2f} GB >> 50 MB L2; {B} distinct topic batches rotated",
                         "matched_ids_per_topic": W["ids"] / n, "matched_filters_per_topic": W["filters"] / n, "visited_nodes_per_topic": W["visited"] / n,
                         "deferred_topics_per_batch": W["deferred"], "probe_diag": diag,
                         "trie": {k: st[k] for k in ("values", "nodes", "edges", "edge_slots", "dict_entries", "plus_nodes", "device_bytes", "max_depth")},

@@ -1,4 +1,4 @@
-/* libgpumqtt — C ABI of the B200-native MQTT topic-filter matching engine.
+/* libgpumqtt — C ABI of the H100-native (sm_90a) MQTT topic-filter matching engine.
  *
  * This is the drop-in boundary for ONE hot path of rmqtt (reference commit 4f9f2185):
  *

@@ -1,4 +1,4 @@
-"""In-tree build of the native libraries (nvcc for sm_100a; g++ for the workload generator).
+"""In-tree build of the native libraries (nvcc for sm_90a; g++ for the workload generator).
 
 The built .so files stay in-tree (git-ignored) so that they travel to the GPU box with the snapshot.
 """
@@ -15,7 +15,7 @@ LIB = PKG / "libgpumqtt.so"
 WL_LIB = PKG / "libgmworkload.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3", "-shared",
 ]
 

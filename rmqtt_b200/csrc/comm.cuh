@@ -6,8 +6,8 @@
 // NCCL has no native all-gatherv: the collective is an ncclAllGather of the per-rank sizes (k topics, m ids)
 // followed by ONE grouped launch of point-to-point transfers (every rank ncclSends its three arrays — topic index, spans,
 // ids, straight out of the buffers the match kernels wrote — to every peer and ncclRecvs theirs into pre-sized contiguous
-// arrays; over NVSwitch every pair has its own full-bandwidth path, measured 2x faster than per-rank ncclBroadcasts at
-// 2 ranks); a small kernel re-bases the received spans.  libnccl is bound at run time (dlopen) so that the library loads, and everything single-GPU
+// arrays; over NVSwitch every pair has its own full-bandwidth path, so the pairs run at once instead of one broadcast
+// root at a time); a small kernel re-bases the received spans.  libnccl is bound at run time (dlopen) so that the library loads, and everything single-GPU
 // works, on hosts without NCCL; inside a torch process the already-loaded libnccl.so.2 is reused.
 #pragma once
 #include <cuda_runtime.h>
@@ -123,8 +123,8 @@ __global__ void k_rebase_spans(uint2* __restrict__ spans, const unsigned long lo
 
 // PUSH form of the peer-memory gather: the match kernels published this rank's rows / ids into ITS OWN block; this kernel
 // copies the slab to the same place in every peer's block with 16-byte loads and stores (NVLink writes in full 128-byte
-// packets, every SM busy), still without a collective call or a host synchronisation.  Measured against the direct form
-// (the publish phase storing every id into all blocks itself): see DESIGN.md §6.
+// packets, every SM busy), still without a collective call or a host synchronisation.  The direct form (the publish
+// phase storing every id into all blocks itself) stays selectable for comparison (debug knob gather_direct).
 __global__ void __launch_bounds__(256)
 k_gather_push(char* const* blocks /* [world] */, u32 rank, u32 world, size_t off_ids, size_t off_spans, size_t off_index,
               unsigned long long base_topics, unsigned long long base_ids, unsigned long long k, const unsigned long long* d_m) {

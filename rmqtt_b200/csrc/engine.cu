@@ -1,4 +1,4 @@
-// libgpumqtt: C ABI (include/gpumqtt.h) over the host mirror (host_trie.cpp) and the sm_100a kernels
+// libgpumqtt: C ABI (include/gpumqtt.h) over the host mirror (host_trie.cpp) and the sm_90a kernels
 // (kernels.cuh).  There is no CPU fallback: without a CUDA device every entry point that would match
 // returns GM_ERR_NO_DEVICE.
 #include <cuda_runtime.h>
@@ -637,7 +637,7 @@ struct gm_engine {
 // =====================================================================================================
 extern "C" {
 
-const char* gm_version(void) { return "libgpumqtt 0.1 (sm_100a)"; }
+const char* gm_version(void) { return "libgpumqtt 0.1 (sm_90a)"; }
 const char* gm_last_error(gm_engine*) { return g_err.c_str(); }
 
 int32_t gm_create(const gm_config* cfg, gm_engine** out) {
@@ -1405,7 +1405,7 @@ int32_t gm_allgatherv_device(gm_engine* e, const uint32_t* d_index, const gm_spa
     if (K > cap_topics || M > cap_ids) { g_err = "gm_allgatherv_device: output too small (sizes[] holds what every rank contributes)"; return GM_ERR_CAPACITY; }
     // 2. one grouped launch, straight out of the buffers the match kernels wrote.  Default: point-to-point (every rank sends
     //    its three arrays to every peer and receives theirs — each pair has its own NVSwitch path); GM_ALLGATHERV=bcast
-    //    selects one ncclBroadcast per (rank, array) instead (A/B, profiles/).
+    //    selects one ncclBroadcast per (rank, array) instead, for comparison.
     std::vector<u64> kof(W + 1, 0), mof(W + 1, 0);
     for (u32 r = 0; r < W; ++r) { kof[r + 1] = kof[r] + sizes[2 * r]; mof[r + 1] = mof[r] + sizes[2 * r + 1]; }
     if (e->knobs.gather_bcast) {

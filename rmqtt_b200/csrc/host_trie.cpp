@@ -57,8 +57,8 @@ HostTrie::HostTrie(u32 max_levels) : max_levels_(max_levels) {
 
 void HostTrie::reserve(u64 n_filters) {
     // ~2.5 edges and ~0.1 new level strings per filter on IoT-shaped sets.  13 slots per filter keeps the edge
-    // table at load ~0.2: measured on C3, 0.38 -> 0.19 shortens the linear probes enough to make the match
-    // kernel 9 % faster (profiles/r1_ab_hints_loadfactor.txt); HBM capacity (180 GB) is not the constraint.
+    // table at load ~0.2: on C3, 0.38 -> 0.19 shortens the linear probes of the match kernel; the table of 10 M
+    // filters stays a few GB, so HBM capacity (80 GB) is not the constraint.
     u64 per_filter = 13;
     if (const char* ev = getenv("GM_EDGE_SLOTS_PER_FILTER")) { int v = atoi(ev); if (v >= 3 && v <= 64) per_filter = static_cast<u64>(v); }   // tuning knob
     u64 want_e = 1; while (want_e < n_filters * per_filter) want_e <<= 1;

@@ -1,9 +1,9 @@
-// sm_100a kernels of the PUBLISH -> matching-subscribers hot path.
+// sm_90a kernels of the PUBLISH -> matching-subscribers hot path.
 //
 //   k_tokenize     Topic::from_str (rmqtt/src/topic.rs:326-363) for a batch: split on '/', classify,
 //                  validate, and intern every level through the device dictionary -> u32 tokens.
 //   k_match_fast   TopicTree::matches (rmqtt/src/trie.rs:299-347, MatchedIter::prepare): one topic per
-//                  thread walks the trie depth-first (one 256-bit load per visited node), then the warp
+//                  thread walks the trie depth-first (one 32-byte load per visited node), then the warp
 //                  publishes its 32 match lists with a scan + load-balanced (ballot/shuffle) expansion:
 //                  single pass, per-topic contiguous output.
 //   k_match_slow   the same walk for the topics the fast path defers (more levels than the fast
@@ -21,7 +21,7 @@ namespace gm {
 
 struct MatchParams {
     TrieView tv;
-    const u32* tok8;     // [n][8]  tokens of levels 0..7, one 32-byte row per topic (one 256-bit load)
+    const u32* tok8;     // [n][8]  tokens of levels 0..7, one 32-byte row per topic (one 32-byte load)
     const u32* tok;      // [tok_levels][n]  levels >= 8 only (level-major; deferred kernel)
     const u32* meta;     // [n]
     u32 n;
@@ -64,13 +64,17 @@ template <int FAST_L, int THREADS> constexpr size_t k2_smem_bytes() { return (2 
 // ------------------------------------------------------------------------------------------------
 // (GM_CPU_EMU: tests/native/emu runs these kernels on the CPU under the sanitizers — the few PTX helpers have plain C++ twins)
 #ifndef GM_CPU_EMU
+// One 32-byte slot (32-byte aligned).  sm_90 has no 256-bit access: two 128-bit halves, issued back to back, which
+// fall into the same 32-byte L2 sector, so a slot still costs one sector of DRAM traffic.
 __device__ __forceinline__ void ld256(const void* p, u32 (&w)[8]) {
-    asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
                  : "l"(p));
 }
 __device__ __forceinline__ void st256(void* p, const u32 (&w)[8]) {
-    asm volatile("st.global.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
+    asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};\n\t"
+                 "st.global.v4.u32 [%0+16], {%5,%6,%7,%8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
 }
 __device__ __forceinline__ u32 lanemask_lt() {
     u32 m;
@@ -87,8 +91,8 @@ inline u32 lanemask_lt() { return (1u << (threadIdx.x & 31u)) - 1u; }
 // K1: tokeniser.  One thread per topic, FOUR text bytes per step: the level text is read with aligned
 // 32-bit loads re-aligned by a funnel shift, '/' and the wildcard characters are found with SWAR zero-byte
 // tests, and the packed key words of the level stay in registers (static indexing) where they are compared
-// directly with the 32-byte dictionary slot.  (Round-1 history: a byte-at-a-time loop packing through shared
-// memory ran ~53 instructions per text byte and was issue bound, profiles/r1_k1_bytewise.ncu-rep.)
+// directly with the 32-byte dictionary slot.  (A byte-at-a-time loop packing through shared memory spends many
+// instructions per text byte and is issue bound.)
 constexpr int TOK_THREADS = 256;
 
 __device__ __forceinline__ u32 swar_zero_bytes(u32 v) { return (v - 0x01010101u) & ~v & 0x80808080u; }   // bit 7 of every zero byte (lowest hit exact)
@@ -285,8 +289,8 @@ k_tokenize(const u8* __restrict__ blob, u32 blob_bytes, u32 readable_bytes, cons
 
 // ------------------------------------------------------------------------------------------------
 // Locality pass.  A uniformly random batch revisits a shared subtree (say the filters below `reg/site/+`)
-// once every few thousand topics — long enough for the cold random stream to evict it from L2 in between
-// (measured L2 read hit rate 33 %).  Regrouping the batch by hash(level 0, level 1) makes the topics that
+// once every few thousand topics — long enough for the cold random stream to evict it from L2 in between.
+// Regrouping the batch by hash(level 0, level 1) makes the topics that
 // share those subtrees run in the same tiles: the second and later visits hit L1/L2.  Counting sort:
 // histogram (in k_tokenize) -> k_bucket_scan -> k_bucket_scatter; order inside a bucket is irrelevant.
 __global__ void __launch_bounds__(1024)
@@ -409,15 +413,14 @@ struct Desc { u32 ref, cnt; };
 //   walk     every thread follows its own topic down the trie: at a node it records the matched value
 //            sets ('#' child always, own values on path exhaustion) as 8-byte descriptors, parks the
 //            '+' child of this depth in its shared-memory column, and descends through the literal
-//            child with ONE 256-bit load; when the literal path ends it resumes the deepest parked
+//            child with ONE 32-byte load; when the literal path ends it resumes the deepest parked
 //            '+' child.  The dependent chain of a thread is one load long per visited node; latency is
 //            hidden by the other ~1.5 K resident threads of the SM.
 //   publish  warp-cooperative: per-lane totals -> warp scan -> one atomic reservation per tile ->
 //            load-balanced expansion of the descriptors (ballot/scan + binary search by shuffle) so
 //            that the id copies out of `values` and into out_ids are coalesced runs.
 //
-// (Round-1 history: a warp-shared ballot-compacted frontier queue ran at 344 warp-instructions per
-//  topic and 45 % issue utilisation — collective overhead, not memory, bound it; see profiles/.)
+// (A warp-shared ballot-compacted frontier queue instead is bound by its collective overhead, not by memory.)
 // DESC = descriptor mode: the publish phase writes each topic's matched value-set references (ref, cnt16) — 8 bytes per
 // matched FILTER instead of 4 bytes per matched id — and spans / cursor / cap count descriptors.  The host resolves
 // them against its mirror of `values` (gm_desc_resolve): this is what DefaultRouter::_matches consumes anyway, one
@@ -510,7 +513,7 @@ k_match_fast(MatchParams p, Desc* __restrict__ dpool, u32 pool_rows) {
                 }
                 // ---- choose the ONE slot this thread loads next: the literal child's first probe slot, else the
                 // deepest parked '+' child (its record names the slot directly).  Both kinds are 32-B edge slots with
-                // the same layout, so all lanes of the warp meet again at a single 256-bit load.
+                // the same layout, so all lanes of the warp meet again at a single 32-byte load.
                 u32 idx = 0, nd = 0, kp = 0, kt = 0;
                 bool probe = false;
                 if (d < L) {
@@ -597,8 +600,8 @@ k_match_fast(MatchParams p, Desc* __restrict__ dpool, u32 pool_rows) {
                 const u32 dst = cur;
                 cur += ni;
                 // load-balanced expansion: flat id index e -> (owner lane, k) by binary search over `exc`.
-                // (A/B, profiles/r1_ab_hints_loadfactor.txt: one cooperative copy per large set + per-lane copies of
-                //  the small ones is 10 % slower — the serial shuffle/copy chain per set costs more than the search.)
+                // (one cooperative copy per large set + per-lane copies of the small ones is slower: the serial
+                //  shuffle/copy chain per set costs more than the search.)
                 u32 sc = ni;
 #pragma unroll
                 for (int o = 1; o < 32; o <<= 1) { u32 v = __shfl_up_sync(0xFFFFFFFFu, sc, o); if (lane >= o) sc += v; }

@@ -1,11 +1,11 @@
-// Data layout shared by the host mirror (host_trie.cpp) and the sm_100a kernels (kernels.cuh).
+// Data layout shared by the host mirror (host_trie.cpp) and the sm_90a kernels (kernels.cuh).
 //
 // The reference keeps the subscription trie as HashMap<Level, Node> per node with a BTreeSet<V> of
 // values (rmqtt/src/trie.rs:69-73).  Here the whole trie lives in HBM as four flat arrays:
 //
 //   dict   : open-addressing table  level string -> u32 token          (32-B slots, string inline)
 //   edges  : open-addressing table  (parent node, token) -> child + the child's *node record*
-//            (32-B slots; ONE 256-bit load answers "does the child exist, what are its values, its
+//            (32-B slots; ONE 32-byte load answers "does the child exist, what are its values, its
 //             '#'-child values, its '+'-child, which tokens can continue below it")
 //   ranges / values : value sets with >1 element (single values are stored inline in the record)
 //
@@ -84,9 +84,8 @@ constexpr u32 WIDE_FANOUT = 48;
 
 
 // ---- windows of the edge table -------------------------------------------------------------------
-// Measured on B200 (tools/randbench5.cu, profiles/r1_randbench_e.txt): random 32-B fetches from a multi-GB
-// table top out at ~37 G/s when every SM roams the whole table, but reach ~48 G/s when each CTA stays inside
-// a window of <= 64 MiB (address-translation reach).  The edge table is therefore cut into `nwin` equal
+// Random 32-B fetches from a multi-GB table run faster when each CTA stays inside a window of <= 64 MiB
+// (address-translation reach) than when every SM roams the whole table.  The edge table is therefore cut into `nwin` equal
 // windows (a power of two): the child edges of a node all live in ONE window, named by the 8-bit tag in the
 // node's record; trie nodes of depth >= 3 inherit the tag of their depth-2 ancestor, so a whole
 // `level0/level1/...` subtree hashes into one window — and since the batch is walked in (level0, level1)

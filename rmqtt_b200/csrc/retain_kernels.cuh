@@ -1,4 +1,4 @@
-// sm_100a kernels of the SUBSCRIBE -> retained-message lookup (RetainTree::matches,
+// sm_90a kernels of the SUBSCRIBE -> retained-message lookup (RetainTree::matches,
 // rmqtt/src/retain.rs:291-367) for a batch of topic filters.
 //
 // A query is a FILTER, so its work is data dependent: an exact filter touches one path, `reg/+/+/...`
@@ -89,7 +89,7 @@ __device__ __forceinline__ void emit_desc(const RetainParams& p, u32 sq, u32 q, 
 // pre-order), not of the warp that produced it.  The next round consumes the slices one after another, so all the tasks
 // that expand the same part of the tree — dozens of filters such as `+/+/+/…` and `reg/+/+/…` cover every site block — run
 // close together in time and share the child blocks and the hash slots of the nodes below through L2, instead of each
-// filter streaming the whole tree from HBM again (measured: 9.75 GB of DRAM reads per C4 batch, L2 hit rate 13 %).
+// filter streaming the whole tree from HBM again.
 __device__ __forceinline__ void push_tasks(const RetainParams& p, RTask* out, u32* n_out, u32, u32 q, u32 pos, u32 mode, u32 kb, u32 kn) {
     const u32 nt = (kn + RTASK_CHUNK - 1) / RTASK_CHUNK;
     if (nt == 0) return;
@@ -206,9 +206,8 @@ k_retain_init(RetainParams p, RTask* out, u32* n_out) {
 // warp walks it in LOCK STEP instead of lane by lane: children whose Bloom mask admits the next level are compacted
 // (ballot) into a per-warp list of node ids in shared memory; the list is then probed 32 nodes per instruction, the
 // nodes that exist and go on form the next list, and so on down the exact run.  Every probe instruction therefore has
-// (nearly) all 32 lanes busy and 32 independent random loads in flight; the lane-by-lane version measured 13.7 of 32
-// active lanes and half the random-access rate of the part (profiles/r2_retain_round_v1.ncu-rep).  Anything that is
-// not an exact level (the next '+', a '#', a stored literal wildcard) goes through retain_chain as before.
+// (nearly) all 32 lanes busy and 32 independent random loads in flight, where a lane-by-lane walk leaves most lanes
+// idle and few loads in flight.  Anything that is not an exact level (the next '+', a '#', a stored literal wildcard) goes through retain_chain as before.
 constexpr u32 RLIST = 256;    // = RTASK_CHUNK: at most one survivor per child of the task
 #ifndef GM_RETAIN_CTAS
 #define GM_RETAIN_CTAS 6

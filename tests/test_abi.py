@@ -29,7 +29,7 @@ def test_every_declared_symbol_is_exported_and_bound():
 
 def test_version_and_shard_fn():
     lib = N.lib()
-    assert b"sm_100a" in lib.gm_version()
+    assert b"sm_90a" in lib.gm_version()
     s = lib.gm_shard_of(b"reg-01/x", 8, 8)
     assert 0 <= s < 8
     assert lib.gm_shard_of(b"reg-01", 6, 8) == s            # only level 0 counts

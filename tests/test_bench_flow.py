@@ -210,7 +210,8 @@ def fake_gpu(monkeypatch):
 
 
 def _ns(**kw):
-    d = dict(gpus=1, steps=3, warmup=3, impl="own", subs=20_000, topics=2_000, batches=2, no_cpu_baseline=False, e2e_steps=None, no_c4=False)
+    d = dict(gpus=1, steps=3, warmup=3, impl="own", subs=20_000, topics=2_000, batches=2, no_cpu_baseline=False, e2e_steps=None, no_c4=False,
+             dump_outputs=None)
     d.update(kw)
     return argparse.Namespace(**d)
 
@@ -247,6 +248,31 @@ def test_run_own_walks_every_leg_and_isolates_the_failing_ones(fake_gpu):
     # C1 / C2 through tools/bench_configs.py and the Zipf batch ride on the fake too (count parity is real: oracle vs oracle-backed fake)
     assert set(d["configs"]) == {"C1", "C2", "C3-zipf"} and d["configs"]["C1"]["count_parity"] is True and d["configs"]["C2"]["count_parity"] is True
     assert d["configs"]["C3-zipf"]["topics_per_s"] > 0
+
+
+def test_dump_outputs_holds_the_last_timed_step(fake_gpu, tmp_path):
+    """--dump-outputs: the lists of the last timed batch (steps=3, batches=2 -> batch 0), every topic's count and a sorted
+    sample, equal to the oracle's; float arrays only, and the same bytes from a second run with the same arguments."""
+    from oracle import oracle as orc
+    from rmqtt_b200 import workload as wl
+    bench, out = fake_gpu
+    bench.run_own(_ns(no_cpu_baseline=True, dump_outputs=str(tmp_path / "a")))
+    d = {f.stem: np.load(f) for f in (tmp_path / "a").glob("*.npy")}
+    assert set(d) == {"counts", "status", "sample_topics", "sample_offsets", "sample_ids"}
+    assert all(a.dtype in (np.float32, np.float64) for a in d.values())
+    cfg = wl.C3.scaled(n_subs=20_000, n_topics=2_000)
+    tree = orc.TopicTree()
+    tree.bulk_insert(*wl.gen_subs(cfg))
+    tb, to = wl.gen_topics(cfg, 2_000, stream=0)
+    want = tree.match_batch(tb, to, want_ids=True)
+    assert (d["counts"] == want["counts"]).all() and len(d["sample_topics"]) == 2_000
+    for i, t in enumerate(d["sample_topics"].astype(np.int64)):
+        o, w = d["sample_offsets"].astype(np.int64), want["offsets"].astype(np.int64)
+        assert (d["sample_ids"][o[i]:o[i + 1]] == np.sort(want["ids"][w[t]:w[t + 1]])).all()
+    bench._EMITTED = False
+    bench.run_own(_ns(no_cpu_baseline=True, dump_outputs=str(tmp_path / "b")))
+    for name, a in d.items():
+        assert np.array_equal(np.load(tmp_path / "b" / f"{name}.npy"), a), name
 
 
 def test_run_own_without_the_cpu_legs(fake_gpu, monkeypatch):

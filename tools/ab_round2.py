@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Round-2 A/B measurements on one B200 (C3): tokeniser with / without the TMA bulk stage, e2e chunk size,
+"""Round-2 A/B measurements on one GPU (C3): tokeniser with / without the TMA bulk stage, e2e chunk size,
 and the retained lookup (C4) with work counters.  One JSON line per measurement on stdout."""
 import ctypes as C
 import json

@@ -1,5 +1,7 @@
 import os, random, sys
-sys.path.insert(0, "/root/repo"); sys.path.insert(0, "/root/repo/tests")
+from pathlib import Path
+_ROOT = Path(__file__).resolve().parent.parent
+sys.path.insert(0, str(_ROOT)); sys.path.insert(0, str(_ROOT / "tests"))
 os.environ["GM_WIN_MIN_SLOTS_LOG2"] = "3"
 from oracle import oracle as orc
 from rmqtt_b200.engine import Engine, GpuMqttError, pack

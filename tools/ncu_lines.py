@@ -15,7 +15,7 @@ top = int(sys.argv[3]) if len(sys.argv) > 3 else 30
 
 tmp = Path(tempfile.mkdtemp())
 subprocess.run(["cuobjdump", "-xelf", "all", str(ROOT / "rmqtt_b200" / "libgpumqtt.so")], cwd=tmp, check=True, stdout=subprocess.DEVNULL)
-dis = subprocess.run(["nvdisasm", "-g", "-c", str(tmp / "engine.sm_100a.cubin")], capture_output=True, text=True).stdout
+dis = subprocess.run(["nvdisasm", "-g", "-c", str(tmp / "engine.sm_90a.cubin")], capture_output=True, text=True).stdout
 addr2line, cur, infn = {}, None, False
 SRC = {}
 for ln in dis.splitlines():

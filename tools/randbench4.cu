@@ -6,13 +6,13 @@
 #include <cstdio>
 template <int HINT> __device__ __forceinline__ void ld256(const void* p, uint32_t (&w)[8]) {
     if (HINT == 128)
-        asm volatile("ld.global.nc.L2::128B.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+        asm volatile("ld.global.nc.L2::128B.v4.u32 {%0,%1,%2,%3}, [%8]; ld.global.nc.L2::128B.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                      : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
     else if (HINT == 64)
-        asm volatile("ld.global.nc.L2::64B.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+        asm volatile("ld.global.nc.L2::64B.v4.u32 {%0,%1,%2,%3}, [%8]; ld.global.nc.L2::64B.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                      : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
     else
-        asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+        asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8]; ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                      : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
 }
 __device__ __forceinline__ uint32_t mix(uint32_t h) { h ^= h >> 16; h *= 0x85EBCA6Bu; h ^= h >> 13; h *= 0xC2B2AE35u; h ^= h >> 16; return h; }
@@ -49,7 +49,7 @@ __global__ void k(const uint4* __restrict__ tab, uint32_t line_mask, int iters, 
     if (acc == 0x12345678u) out[0] = acc;
 }
 template <int NS, int HINT, bool DEP> void run(const uint4* tab, size_t bytes, uint32_t* out) {
-    int iters = 64, blocks = 148 * 4, threads = 512;
+    int iters = 64, blocks = [] { cudaDeviceProp p; cudaGetDeviceProperties(&p, 0); return p.multiProcessorCount; }() * 4, threads = 512;
     uint32_t mask = uint32_t(bytes / 128) - 1;
     cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
     k<NS, HINT, DEP><<<blocks, threads>>>(tab, mask, iters, out);
