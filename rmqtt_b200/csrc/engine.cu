@@ -1702,8 +1702,14 @@ int32_t gm_debug_table(gm_engine* e, uint32_t which, const void** ptr, uint64_t*
 
 int32_t gm_debug_knob(gm_engine* e, const char* name, int64_t value) {
     if (!e || !name) return GM_ERR_INVALID_ARG;
-    std::lock_guard<std::mutex> g(e->mu_dev);
     const std::string k(name);
+    if (k == "retain_caps") {     // scratch of the retained lookup (items / descriptors, over all RQ slices); run_retain grows it on overflow
+        if (value < int64_t(RQ) || value % RQ != 0 || value > (int64_t(1) << 30)) return GM_ERR_INVALID_ARG;
+        std::lock_guard<std::mutex> gr(e->mu_ret);          // (mu_ret before mu_dev: the lock order of the retained lookup)
+        e->r_cap_items = e->r_cap_desc = static_cast<u32>(value);
+        return GM_OK;
+    }
+    std::lock_guard<std::mutex> g(e->mu_dev);
     if (k == "tile_chunk" && value >= 1 && value <= 1024) e->knobs.tile_chunk = static_cast<u32>(value);
     else if (k == "k2_ctas" && value >= 0 && value <= 8) e->knobs.k2_ctas = static_cast<int>(value);
     else if (k == "sorted_rows") e->knobs.sorted_rows = value != 0;

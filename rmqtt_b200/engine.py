@@ -426,7 +426,12 @@ class Engine:
         return out
 
     def debug_knob(self, name: str, value: int) -> None:
-        """Set a kernel-scheduling knob (gm_debug_knob): tuning / A-B measurements only, results never change."""
+        """Set a kernel-scheduling knob (gm_debug_knob): tuning / A-B measurements only, results never change.
+
+        tests/test_gpu_edges.py holds these to that promise against the oracle: tok_bulk, sorted_rows, tile_chunk (1..1024),
+        k2_ctas (0 = default, 1..3), bucket_bits (site bits * 100 + sub bits, sum <= 18), small_graphs, e2e_chunk (>= 1024
+        topics per pipelined chunk) and retain_caps (starting size of the retained lookup's scratch, a multiple of 64 that is
+        at least 64; the lookup grows it when a batch overflows it)."""
         self._check(self._lib.gm_debug_knob(self._h, name.encode(), int(value)))
 
     def kernel_ms(self, max_calls: int = 64) -> np.ndarray:

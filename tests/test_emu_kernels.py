@@ -830,6 +830,66 @@ def test_value_set_size_boundary_wide_nodes_tiny_windows_and_an_empty_spill_pool
     e.close()
 
 
+def _emu_load_corpus(emu, e, c):
+    emu.emu_bulk_load.restype = C.c_uint64
+    for f, v in c.adds:
+        assert e.add(f, v) == 0, f
+    for f, v0, k in c.bulk:
+        fb, fo = pack([f] * k)
+        vals = np.arange(v0, v0 + k, dtype=np.uint32)
+        assert emu.emu_bulk_load(e.h, C.c_void_p(fb.ctypes.data), C.c_void_p(fo.ctypes.data), C.c_void_p(vals.ctypes.data), C.c_uint64(k)) == k
+    for tr, fl in c.trees.items():
+        for f, v in fl:
+            assert e.add(f, v, tree=tr) == 0
+
+
+def test_boundary_corpus_reaches_its_paths(emu, monkeypatch):
+    """The boundary corpus of tests/_edges.py (also run on the GPU by tests/test_gpu_edges.py) with the spill pool at the GPU's
+    24 rows: parity with the oracle in ids / descriptor mode, plain / bulk-staged tokeniser, and the instrumented kernels'
+    V / E / F / M; the number of deferred topics is exactly the corpus's count — so every case reaches the path it is meant
+    for (8 / 9 / 32 / 33 matched sets, 65534 / 65535-member sets, 8 / 9 levels) before any GPU time is spent."""
+    import _edges as E
+    c = E.subscription_corpus()
+    trees = c.tree_oracles()
+    E.check_against_oracle(c, trees[0])
+    e = Emu(emu)
+    emu.emu_set_pool_rows(e.h, E.K2_POOL_ROWS)
+    _emu_load_corpus(emu, e, c)
+    for name in ("main", "big_tile", "huge", "stage", "n33", "n513"):
+        tb, to = c.packed(name)
+        want = trees[0].match_batch(tb, to)
+        for flags in (0, 1, 2, 4):
+            res, work, deferred = e.match(tb, to, flags)
+            _same(res, want)
+            assert (res.status == np.where(want["counts"] < 0, -2, 0)).all()
+            assert deferred == c.n_deferred(name), (name, flags)
+            if flags & 4:
+                cnt = want["counters"]
+                assert [int(x) for x in work] == [cnt["V"], cnt["E"], cnt["F"], cnt["M"]], name
+    tb, to = c.packed("main")                                   # rows of other trees, one that does not exist
+    rows = np.asarray([(0, 1, 5, 9)[i % 4] for i in range(len(to) - 1)], dtype=np.uint32)
+    res, _, _ = e.match(tb, to, 0, trees=rows)
+    for i, x in enumerate(c.batches["main"]):
+        want = None if x.F is None else sorted(trees[int(rows[i])].matches(x.topic)) if int(rows[i]) in trees else []
+        assert res.sorted_list(i) == want, (x.topic, rows[i])
+    e.close()
+    monkeypatch.setenv("GM_WIN_MIN_SLOTS_LOG2", "3")            # 8-slot windows: probes wrap, the tables re-hash as they fill
+    s = E.subscription_corpus(shallow=True)
+    e = Emu(emu)
+    emu.emu_set_pool_rows(e.h, E.K2_POOL_ROWS)
+    _emu_load_corpus(emu, e, s)
+    tb, to = s.packed("main")
+    want = s.load_oracle().match_batch(tb, to)
+    for flags in (0, 1, 6):
+        res, work, deferred = e.match(tb, to, flags)
+        _same(res, want)
+        assert deferred == 0                                    # 12-level topics, but the trie is 3 levels deep
+        if flags & 4:
+            cnt = want["counters"]
+            assert [int(x) for x in work] == [cnt["V"], cnt["E"], cnt["F"], cnt["M"]]
+    e.close()
+
+
 def test_retained_lookup_beyond_the_eight_level_token_row(emu):
     """Retained topics and filters of up to 14 levels (levels >= 8 live in the level-major token array), literal '+' / '#' levels
     that shadow wildcard expansion, `$` roots, removals — scratch starting small."""
