@@ -189,7 +189,8 @@ int32_t gm_retain_bulk_load(gm_engine* e, const char* blob, const uint32_t* offs
                             uint64_t n, uint64_t* n_set);
 /* Batch removal under ONE lock acquisition — the expiry sweep (remove_expired_messages / RetainTree::retain,
  * rmqtt/src/retain.rs:118-128, 261-288: the host decides which retained topics expired).  old_values (optional, [n]) receives
- * the removed handle or 0xFFFFFFFF where nothing was stored; invalid topics are skipped.                                        */
+ * the removed handle or 0xFFFFFFFF where nothing was stored; invalid topics are skipped.  A stored handle of 0xFFFFFFFF is
+ * therefore indistinguishable from "nothing stored" in old_values: *n_removed is the count to trust.                          */
 int32_t gm_retain_remove_batch(gm_engine* e, const char* blob, const uint32_t* offsets /* n+1 */, uint64_t n, uint32_t* old_values,
                                uint64_t* n_removed);
 /* RetainStorage::get (rmqtt/src/retain.rs:152-169 -> RetainTree::matches :291-367) for a batch of SUBSCRIBE topic

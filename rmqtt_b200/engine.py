@@ -201,7 +201,8 @@ class Engine:
         return int(old.value) if had.value else None
 
     def retain_remove_batch(self, blob: np.ndarray, offs: np.ndarray):
-        """-> (old handles uint32[n] with 0xFFFFFFFF where nothing was stored, number removed)"""
+        """-> (old handles uint32[n] with 0xFFFFFFFF where nothing was stored, number removed).  A stored handle of
+        0xFFFFFFFF looks the same as "nothing stored" in the first array; the number removed is the count to trust."""
         n = len(offs) - 1
         old = np.empty(n, dtype=np.uint32)
         cnt = C.c_uint64(0)

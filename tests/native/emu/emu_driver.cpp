@@ -71,6 +71,8 @@ struct EmuEngine {
     u64 up_values_epoch = 0;
     TrieView dev_view{}; RetainView dev_rview{};
     u64 flushes = 0;
+    std::vector<u64> last_tasks;         // the last successful retained lookup: tasks queued per round (entry 0 = k_retain_init)
+    u64 last_n_desc = 0;                 // ... and descriptors emitted
 
     bool flush() {                       // engine.cu gm_engine::flush_impl, shipping policy only
         if (!trie.any_dirty() && !rtree.dirty && flushes) return true;
@@ -490,8 +492,30 @@ int32_t emu_retain_match(void* h, const char* blob_in, const uint32_t* offs, uin
     emu::launch(dim3(EMU_SMS * 8), dim3(256), [&] { k_retain_expand(rdescs.data(), ctl.n_desc, slice_desc, rv.vals, qbase, qcur, out_ids, cap_ids); });
     if (work) { work[0] = ctl.stats[0]; work[1] = ctl.stats[1]; }
     if (ctl.err) return -100 - static_cast<int32_t>(ctl.err);      // scratch overflow: bit 0 tasks, bit 1 descriptors (the engine grows and retries)
+    e.last_tasks.assign(depth + 2, 0);                             // the totals of engine.cu's `retain stats` line
+    for (u32 l = 0; l <= depth + 1; ++l) for (u32 k = 0; k < RQ; ++k) e.last_tasks[l] += counts[static_cast<size_t>(l) * RQ + k];
+    e.last_n_desc = 0;
+    for (u32 k = 0; k < RQ; ++k) e.last_n_desc += ctl.n_desc[k];
     *needed = ctl.grand;
     return ctl.grand > cap_ids ? -3 : 0;
+}
+
+// tasks queued per round by the last successful emu_retain_match (entry 0 = k_retain_init, entry l + 1 = round l) into
+// out[0 .. cap); returns the number of rounds + 1 (max_depth + 2); *n_desc = the descriptors it emitted
+uint32_t emu_retain_last_tasks(void* h, uint64_t* out, uint32_t cap, uint64_t* n_desc) {
+    const EmuEngine& e = *static_cast<EmuEngine*>(h);
+    for (size_t l = 0; l < e.last_tasks.size() && l < cap; ++l) out[l] = e.last_tasks[l];
+    if (n_desc) *n_desc = e.last_n_desc;
+    return static_cast<uint32_t>(e.last_tasks.size());
+}
+// the host image of the retained tree (gm_debug_table 7 = rnodes, 8 = rkids: 8 words per entry)
+int32_t emu_retain_table(void* h, uint32_t which, const void** ptr, uint64_t* count) {
+    RetainTreeHost& t = static_cast<EmuEngine*>(h)->rtree;
+    t.prepare_flush();
+    if (which == 7) { *ptr = t.rnodes.data(); *count = t.rnodes.size(); }
+    else if (which == 8) { *ptr = t.rkids.data(); *count = t.rkids.size(); }
+    else return -1;
+    return 0;
 }
 
 // gm_relations_expand_device over host arrays (k_relations)

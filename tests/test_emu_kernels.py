@@ -98,6 +98,8 @@ class Emu:
             return MatchResult(spans, ids[:int(needed.value)], status, int(needed.value)), work, int(deferred.value)
 
     def retain_match(self, blob, offs, stats=0, cap_items=1 << 14, cap_desc=1 << 14):
+        """-> (MatchResult, work, attempts that overflowed); self.errs = the overflow bits of each of them"""
+        self.errs = []
         n = len(offs) - 1
         spans = np.zeros((n, 2), dtype=np.uint32)
         status = np.zeros(n, dtype=np.int32)
@@ -114,6 +116,7 @@ class Emu:
                 continue
             if rc <= -100:                       # scratch overflow bits: grow like gm_engine::run_retain does
                 err = -rc - 100
+                self.errs.append(err)
                 cap_items *= 4 if err & 1 else 1
                 cap_desc *= 4 if err & 2 else 1
                 grew += 1
@@ -121,6 +124,23 @@ class Emu:
                 continue
             assert rc == 0, rc
             return MatchResult(spans, ids[:int(needed.value)], status, int(needed.value)), work, grew
+
+
+    def retain_tasks(self):
+        """-> (tasks queued per round by the last retained lookup, entry 0 = k_retain_init; descriptors emitted)"""
+        out, nd = np.zeros(256, dtype=np.uint64), C.c_uint64(0)
+        k = self.lib.emu_retain_last_tasks(self.h, C.c_void_p(out.ctypes.data), 256, C.byref(nd))
+        return [int(x) for x in out[:k]], int(nd.value)
+
+    def retain_image(self):
+        """(rnodes, rkids) of the retained tree's image, 8 words per entry (Engine.debug_tables() layout)"""
+        out = []
+        for which in (7, 8):
+            ptr, cnt = C.c_void_p(), C.c_uint64(0)
+            assert self.lib.emu_retain_table(self.h, which, C.byref(ptr), C.byref(cnt)) == 0
+            n = int(cnt.value) * 8
+            out.append(np.frombuffer((C.c_uint32 * n).from_address(ptr.value), dtype=np.uint32).copy().reshape(-1, 8) if n else np.zeros((0, 8), np.uint32))
+        return out
 
 
 def _canon(want):
@@ -307,6 +327,7 @@ T.test_partition_kernel_equals_the_host_shard_function(lib)
 T.test_fused_gather_over_emulated_peer_memory(lib, 3, 0)
 T.test_fused_gather_over_emulated_peer_memory(lib, 3, 1)
 T.test_relation_expansion_kernel_against_a_python_model(lib)
+T._emu_retained_corpus(lib, "bulk", asan=True)
 print("asan run ok")
 """)
     libasan = subprocess.run(["g++", "-print-file-name=libasan.so"], capture_output=True, text=True).stdout.strip()
@@ -923,4 +944,161 @@ def test_retained_lookup_beyond_the_eight_level_token_row(emu):
     res, _, grew = e.retain_match(fb, fo, cap_items=256, cap_desc=256)
     assert grew >= 1
     _same(res, rt.match_batch(fb, fo))
+    e.close()
+
+
+# ---- the retained boundary corpus (tests/_retain_edges.py) --------------------------------------------------------------------
+class _Env:
+    """Environment variables of the host builders for one block (the emulated library reads them in this process)."""
+
+    def __init__(self, **kv):
+        self.kv, self.old = kv, {}
+
+    def __enter__(self):
+        import os
+        for k, v in self.kv.items():
+            self.old[k] = os.environ.get(k)
+            os.environ[k] = str(v)
+
+    def __exit__(self, *a):
+        import os
+        for k, v in self.old.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+
+
+def _emu_retained_load(lib, e, c, how):
+    """(a) "set": retain_set one by one (the first lookup flattens), the 65537-child node by retain_bulk_load into the
+    non-empty tree; (b) "bulk": everything in one retain_bulk_load into the empty tree, down the parallel level-by-level build."""
+    lib.emu_retain_bulk_load.restype = C.c_uint64
+    if how == "set":
+        for t, v in c.sets:
+            assert e.retain_set(t, v) == 0, t
+        todo = c.bulk
+    else:
+        todo = c.all_topics()
+    if todo:
+        tb, to = pack([t for t, _ in todo])
+        vals = np.asarray([v for _, v in todo], dtype=np.uint32)
+        with _Env(GM_HOST_PAR_MIN=1, GM_HOST_THREADS=4):
+            assert lib.emu_retain_bulk_load(e.h, C.c_void_p(tb.ctypes.data), C.c_void_p(to.ctypes.data), C.c_void_p(vals.ctypes.data), C.c_uint64(len(vals))) == len(vals)
+
+
+def _emu_rstats(lib, e):
+    ctr = np.zeros(6, dtype=np.uint64)
+    lib.emu_retain_counters(e.h, C.c_void_p(ctr.ctypes.data))
+    return int(ctr[0]), int(ctr[1])            # full rebuilds, in-place patches
+
+
+def _emu_retained_same(e, rt, filters, caps, what):
+    fb, fo = pack(filters)
+    res, _, _ = e.retain_match(fb, fo, cap_items=caps, cap_desc=caps)
+    want = rt.match_batch(fb, fo)
+    try:
+        _same(res, want)
+        assert (res.status == np.where(want["counts"] < 0, -2, 0)).all()
+    except AssertionError as ex:
+        raise AssertionError(f"{what}: {ex}") from None
+    return res
+
+
+def _emu_retained_checks(e, c, rt, caps, heavy=True, batches=()):
+    """The filters in one batch; every stated case alone with its tasks per round; the batch shapes."""
+    _emu_retained_same(e, rt, c.filters(heavy), caps, "all filters")
+    for q in c.stated():
+        if q.heavy and not heavy:
+            continue
+        _emu_retained_same(e, rt, [q.filt], caps, q.filt)
+        got, _ = e.retain_tasks()
+        assert len(got) >= len(q.tasks) and got == list(q.tasks) + [0] * (len(got) - len(q.tasks)), (q.filt, got, q.tasks)
+    for n in batches:
+        _emu_retained_same(e, rt, c.batch(n), caps, f"batch of {n}")
+
+
+def _emu_retained_corpus(lib, how, asan=False):
+    """Both corpora in one loading: at the default scratch, then from 64 entries (one per queue slice; the heavy cases stay at
+    the default: from 64 entries `w/k65537/+` alone needs 11 growths, one queue kind at a time)."""
+    import _retain_edges as R
+    R.check_constants()
+    for c in (R.retained_edge_corpus(), R.retained_lit_hash_corpus()):
+        e, rt = Emu(lib), c.load_oracle(orc)
+        _emu_retained_load(lib, e, c, how)
+        if asan:                                     # the nesting and mode-2 cases (the in-place stack) and the light batch
+            _emu_retained_same(e, rt, c.filters(heavy=False), 1 << 14, "all light filters")
+            for q in c.stated():
+                if q.filt.startswith(("n/", "h/")):
+                    _emu_retained_same(e, rt, [q.filt], R.RQ, q.filt)
+                    assert e.retain_tasks()[0][:len(q.tasks)] == list(q.tasks), q.filt
+            e.close()
+            continue
+        _emu_retained_checks(e, c, rt, 1 << 14, batches=(1, 255, 256, 257, 1025) if how == "bulk" and c.bulk else ())
+        _emu_retained_checks(e, c, rt, R.RQ, heavy=False, batches=(257,) if how == "bulk" and c.bulk else ())
+        if c.bulk:
+            img = R.Image(*e.retain_image())
+            R.bloom_proof(c, img)
+            R.root_interleave_proof(c, img)
+        e.close()
+
+
+@pytest.mark.parametrize("how", ["set", "bulk"])
+def test_retained_corpus_boundaries(emu, how):
+    """The retained boundary corpus loaded (a) one by one or (b) in bulk, at the default scratch and from a 64-entry scratch:
+    bit-exact against the oracle, every shape case queues exactly the tasks it states, and the Bloom-mask and root-order
+    cases are proved from the image.  (The batches of 1023 .. 4097 filters run on the GPU, tests/test_gpu_retain_edges.py.)"""
+    _emu_retained_corpus(emu, how)
+
+
+def test_retained_corpus_scratch_overflow_grows_only_the_queue_that_overflowed(emu):
+    """From 64 entries (one per slice): `w/k513/+/zz` queues 3 tasks into one slice and emits nothing -> only the task queue
+    overflows; `pi/+` emits 3 values into one slice and queues nothing -> only the descriptor list.  Each grows once."""
+    import _retain_edges as R
+    c = R.retained_edge_corpus()
+    e, rt = Emu(emu), c.load_oracle(orc)
+    _emu_retained_load(emu, e, c, "bulk")
+    for f, bits in (("w/k513/+/zz", [1]), ("pi/+", [2]), ("pi/+/k", [2])):
+        _emu_retained_same(e, rt, [f], R.RQ, f)
+        assert e.errs == bits, (f, e.errs)
+    e.close()
+
+
+def test_retained_corpus_in_place_edits(emu):
+    """(c) the bulk-built image edited in place by the corpus's edit script, every edit checked against the oracle; the
+    full-rebuild / patch counters show which edits stayed in place."""
+    import _retain_edges as R
+    c = R.retained_edge_corpus()
+    e, rt = Emu(emu), c.load_oracle(orc)
+    emu.emu_compact.restype = C.c_int32
+    _emu_retained_load(emu, e, c, "bulk")
+    _emu_retained_same(e, rt, ["#"], 1 << 14, "first lookup")
+    proof = R.bloom_proof(c, R.Image(*e.retain_image()))
+    filters = R.edit_filters(c)
+    for label, op, arg, how in R.edit_script(proof["clear"][0]):
+        before = _emu_rstats(emu, e)
+        if op == "set":
+            assert e.retain_set(*arg) == 0
+            rt.insert(*arg)
+        elif op == "remove":
+            assert e.retain_remove(arg) == 0
+            rt.remove(arg)
+        elif op == "remove_batch":                   # (gm_retain_remove_batch is this loop; the GPU tier calls it)
+            removed = 0
+            for t in arg:
+                if orc.topic_parse(t) is None:
+                    assert e.retain_remove(t) != 0
+                    continue
+                assert e.retain_remove(t) == 0
+                removed += rt.remove(t) is not None
+            assert removed == R.REMOVE_BATCH_REMOVED
+        else:
+            assert emu.emu_compact(e.h) == 0
+        _emu_retained_same(e, rt, filters, 1 << 14, label)
+        after = _emu_rstats(emu, e)
+        if how == "patch":
+            assert after[0] == before[0] and after[1] > before[1], (label, before, after)
+        elif how == "flatten":
+            assert after[0] == before[0] + 1, (label, before, after)
+    _emu_retained_same(e, rt, c.filters() + ["#", "+/#", "$c/#"], 1 << 14, "all filters after the edits")
+    _emu_retained_same(e, rt, filters + c.filters(heavy=False), R.RQ, "from 64 entries after the edits")
     e.close()
