@@ -4,7 +4,7 @@ Every case reaches its boundary by construction and states what it expects: for 
 nodes F (None: Topic::from_str fails) and whether k_match_fast must hand it to the deferred kernel.  `check_against_oracle`
 re-derives F from the oracle one topic at a time, so the corpus cannot drift away from the boundaries it claims to hit.
 
-The constants mirror rmqtt_b200/csrc (kernels.cuh, layout.h, engine.cu); the tests assert the byte counts that depend on them.
+The constants mirror rmqtt_b200/csrc (kernels.cuh, layout.h, pipeline.cuh); the tests assert the byte counts that depend on them.
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ import numpy as np
 from oracle import oracle as orc
 
 K2_SMEM_DESCS = 8            # matched value sets per topic in shared memory (kernels.cuh)
-K2_POOL_ROWS = 24            # ... plus the spill rows in global memory before the topic is deferred (engine.cu)
+K2_POOL_ROWS = 24            # ... plus the spill rows in global memory before the topic is deferred (pipeline.cuh)
 K2_FAST_L = 8                # levels k_match_fast walks; deeper topics are deferred
 CNT_BIG = 0xFFFF             # a value set of >= 65535 members goes through `ranges` (deferred kernel only)
 DICT_INLINE_MAX = 27         # level strings up to 27 bytes live in the dictionary slot, longer ones in the pool

@@ -1,40 +1,61 @@
-// TEST INFRASTRUCTURE: the match and retained-lookup pipelines of engine.cu (enqueue_match / enqueue_retain) over HOST
-// memory, with the REAL kernel sources (kernels.cuh, retain_kernels.cuh, relations.cuh compiled with -DGM_CPU_EMU) run
-// by the CPU emulation in cuda_runtime.h.  Exposed as a small C interface for tests/test_emu_kernels.py, which compares
-// the results with the oracle.  Build (tests/test_emu_kernels.py does it):
+// TEST INFRASTRUCTURE: the match and retained-lookup pipelines over HOST memory.  The launch sequences, scratch plan, views
+// and shipping decisions are engine.cu's own (rmqtt_b200/csrc/pipeline.cuh); the REAL kernel sources (kernels.cuh,
+// retain_kernels.cuh, relations.cuh compiled with -DGM_CPU_EMU) run on the CPU emulation in cuda_runtime.h.  What stays here
+// is what the engine does around a launch (staging, the device image a flush keeps) and the test-only checks.  Exposed as a
+// small C interface for tests/test_emu_kernels.py, which compares the results with the oracle.  Build (the test does it):
 //   g++ -O1 -g -std=c++17 -DGM_CPU_EMU -Itests/native/emu -Irmqtt_b200/csrc -shared -fPIC tests/native/emu/emu_driver.cpp \
 //       rmqtt_b200/csrc/host_trie.cpp rmqtt_b200/csrc/retain_tree.cpp -o <out>.so     (+ -fsanitize=address,undefined for the ASan run)
 #include <cuda_runtime.h>      // the emulation (this directory is first on the include path)
 
 #include <cstring>
+#include <new>
 #include <vector>
 
-#include "../../../include/gpumqtt.h"
 #include "comm.cuh"
-#include "host_trie.h"
-#include "kernels.cuh"
+#include "pipeline.cuh"
 #include "relations.cuh"
-#include "retain_kernels.cuh"
-#include "retain_tree.h"
 
 using namespace gm;
 
 namespace {
 
-struct Ctrl { unsigned long long cursor; unsigned long long stats[24]; u32 slow_count; u32 tile_counter; };   // engine.cu's control block
-
-constexpr int K2_FAST_L = 8, K2_THREADS = 512, K2_CTAS_PER_SM = 3;
 constexpr u32 EMU_SMS = 2;               // the emulated part has two SMs: several CTAs per kernel, dynamic tile hand-out exercised
 
-// A "device copy" of one table, maintained ONLY by what gm_engine::flush_impl would ship (engine.cu upload_table /
-// upload_appendable / stage_patches): whole arrays after a re-hash or for the first shipment, appended tails, and the slots the
-// host mirror listed as dirty.  A slot the mirror changed without listing it stays stale here — and shows up as a wrong match.
+// host memory standing in for cudaMalloc'd scratch: zeroed, 256-byte aligned, exactly the planned size (ASan sees its end)
+struct Arena {
+    std::vector<void*> blocks;
+    Arena() = default;
+    Arena(const Arena&) = delete;
+    Arena& operator=(const Arena&) = delete;
+    ~Arena() { for (void* p : blocks) ::operator delete(p, std::align_val_t(256)); }
+    template <class T> T* get(size_t bytes) {
+        void* p = ::operator new(std::max<size_t>(bytes, 1), std::align_val_t(256));
+        std::memset(p, 0, bytes);
+        blocks.push_back(p);
+        return static_cast<T*>(p);
+    }
+};
+
+// a batch's text, 16-byte aligned and readable up to the next 16-byte boundary (what the bulk tokeniser may read)
+struct Text {
+    std::vector<u8> store;
+    u8* p;
+    u32 bytes, readable;
+    Text(const char* src, u32 n) : store((static_cast<size_t>(n) + 15) / 16 * 16 + 64, 0), bytes(n), readable((n + 15u) & ~15u) {
+        p = store.data() + ((16 - (reinterpret_cast<uintptr_t>(store.data()) & 15)) & 15);
+        std::memcpy(p, src, n);
+    }
+};
+
+// A "device copy" of one table, maintained ONLY by what gm_engine::flush_impl would ship (pipeline.cuh ship_table_whole /
+// ship_appendable_fresh): whole arrays, appended tails, and the slots the host mirror listed as dirty.  A slot the mirror
+// changed without listing it stays stale here — and shows up as a wrong match.
 template <class T> struct ImgBuf {
-    std::vector<T> v;                    // v.size() plays the role of DevBuf::cap (elements)
+    std::vector<T> v;                    // v.size() * sizeof(T) plays the role of DevBuf::cap
     size_t up = 0;                       // shipped up to here (appendable arrays) / shipped size (tables)
     bool have = false;
-    template <class H> void fresh(const H& host, size_t min_elems) {
-        v.assign(std::max(std::max(host.size(), min_elems), size_t(8)), T{});
+    template <class H> void fresh(const H& host, size_t min_bytes, size_t slack_bytes = 0) {
+        v.assign((fresh_bytes(host.size() * sizeof(T), min_bytes, slack_bytes) + sizeof(T) - 1) / sizeof(T), T{});
         std::memset(static_cast<void*>(v.data()), 0xCD, v.size() * sizeof(T));          // never-shipped bytes are garbage on a device
         if (host.size()) std::memcpy(static_cast<void*>(v.data()), host.data(), host.size() * sizeof(T));
         up = host.size(); have = true;
@@ -44,12 +65,13 @@ template <class T> struct ImgBuf {
         dirty.clear();
     }
     template <class H> void table(const H& host, bool& full, std::vector<u32>& dirty) {       // engine.cu upload_table
-        if (full || !have || up != host.size() || dirty.size() * 8 > host.size()) { fresh(host, 0); dirty.clear(); }
+        if (ship_table_whole(full, up, host.size(), dirty.size())) { fresh(host, 0); dirty.clear(); }
         else patch(host, dirty);
         full = false;
     }
     template <class H> void appendable(const H& host, std::vector<u32>* dirty) {              // engine.cu upload_appendable
-        if ((up == 0 && (host.size() > 0 || !have)) || host.size() > v.size()) { fresh(host, std::max(host.size() * 2, size_t(1024))); if (dirty) dirty->clear(); return; }
+        const size_t bytes = host.size() * sizeof(T);
+        if (ship_appendable_fresh(up, bytes, have, v.size() * sizeof(T))) { fresh(host, appendable_room(bytes)); if (dirty) dirty->clear(); return; }
         const size_t before = up;
         if (host.size() > up) { std::memcpy(static_cast<void*>(v.data() + up), host.data() + up, (host.size() - up) * sizeof(T)); up = host.size(); }
         if (dirty) {
@@ -62,7 +84,7 @@ template <class T> struct ImgBuf {
 struct EmuEngine {
     HostTrie trie{128};
     RetainTreeHost rtree{&trie};
-    u32 pool_rows = 24;                  // engine.cu K2_POOL_ROWS (tests lower it to push topics onto the deferred kernel)
+    u32 pool_rows = K2_POOL_ROWS;        // (tests lower it to push topics onto the deferred kernel)
     u32 site_bits = 10;
     // optional device image (emu_use_image): the kernels then read copies that only flush() updates
     bool image = false, manual_flush = false;
@@ -80,7 +102,7 @@ struct EmuEngine {
         if (trie.values_epoch != up_values_epoch) { i_values.up = i_ranges.up = 0; up_values_epoch = trie.values_epoch; }
         if (rtree.dirty || !flushes) {
             rtree.prepare_flush();
-            if (rtree.full || !i_rkids.have) { i_rkids.fresh(rtree.rkids, rtree.rkids.size() + rtree.rkids.size() / 4 + 1024); i_redges.fresh(rtree.redges, 0); i_rvals.fresh(rtree.rvals, rtree.rvals.size() + 1024); }
+            if (rtree.full || !i_rkids.have) { i_rkids.fresh(rtree.rkids, 0, retained_kids_slack(rtree.rkids.size())); i_redges.fresh(rtree.redges, 0); i_rvals.fresh(rtree.rvals, 0, RETAINED_VALS_SLACK); }
             else {
                 bool full_edges = false;
                 i_rkids.appendable(rtree.rkids, &rtree.dirty_kids);
@@ -97,11 +119,8 @@ struct EmuEngine {
         if (trie.cfilter_dirty || !i_cfilter.have) { i_cfilter.fresh(trie.cfilter, 0); trie.cfilter_dirty = false; }
         if (trie.trees_dirty || !i_tree_slots.have) { i_tree_slots.fresh(trie.tree_slots, 0); trie.trees_dirty = false; }
         trie.root_dirty = false;
-        dev_view = host_view();
-        dev_view.edges = i_edges.v.data(); dev_view.ranges = i_ranges.v.data(); dev_view.values = i_values.v.data(); dev_view.dict = i_dict.v.data();
-        dev_view.pool = i_pool.v.data(); dev_view.cfilter = i_cfilter.v.data(); dev_view.tree_slots = i_tree_slots.v.data();
-        dev_rview = host_rview();
-        dev_rview.kids = i_rkids.v.data(); dev_rview.edges = i_redges.v.data(); dev_rview.vals = i_rvals.v.data();
+        dev_view = trie_view(trie, i_edges.v.data(), i_ranges.v.data(), i_values.v.data(), i_dict.v.data(), i_pool.v.data(), i_cfilter.v.data(), i_tree_slots.v.data());
+        dev_rview = retain_view(rtree, i_rkids.v.data(), i_redges.v.data(), i_rvals.v.data());
         flushes++;
         return true;
     }
@@ -112,29 +131,24 @@ struct EmuEngine {
         if (!manual_flush || !flushes) return flush();
         return true;
     }
-    TrieView view() { return image ? dev_view : host_view(); }
-    RetainView rview() { return image ? dev_rview : host_rview(); }
-
-    TrieView host_view() {               // engine.cu gm_engine::view(), host pointers instead of device pointers
-        TrieView v{};
-        v.edges = trie.edges.data(); v.ranges = trie.ranges.data(); v.values = trie.values.data(); v.dict = trie.dict.data(); v.pool = trie.pool.data();
-        v.cfilter = trie.cfilter.data(); v.cfilter_mask = static_cast<u32>(trie.cfilter.size() - 1);
-        v.edge_mask = static_cast<u32>(trie.edges.size() - 1);
-        v.win_mask = trie.win_mask(); v.win_shift = trie.win_shift(); v.nwin_mask = trie.nwin_mask();
-        v.dict_mask = static_cast<u32>(trie.dict.size() - 1);
-        v.root_plus = trie.root_plus; v.root_hash_ref = trie.root_hash_ref; v.root_hash_cnt = trie.root_hash_cnt; v.root_mask = trie.root_mask;
-        v.max_depth = trie.max_depth;
-        v.tree_slots = trie.tree_slots.data(); v.n_trees = static_cast<u32>(trie.tree_slots.size());
-        return v;
+    TrieView view() {
+        if (image) return dev_view;
+        return trie_view(trie, trie.edges.data(), trie.ranges.data(), trie.values.data(), trie.dict.data(), trie.pool.data(), trie.cfilter.data(), trie.tree_slots.data());
     }
-    RetainView host_rview() {            // engine.cu gm_engine::rview()
-        RetainView v{};
-        v.kids = rtree.rkids.data(); v.edges = rtree.redges.data(); v.vals = rtree.rvals.data();
-        v.edge_mask = static_cast<u32>(rtree.redges.size() - 1);
-        if (!rtree.rnodes.empty()) { v.root_first_kid = rtree.rnodes[0].first_kid; v.root_nk_flags = rtree.rnodes[0].nkids | (rtree.rnodes[0].flags << 28); }
-        v.root_plain_kids = rtree.root_plain_kids; v.root_plain_val_hi = rtree.root_plain_val_hi; v.max_depth = rtree.max_depth;
-        v.n_kids = static_cast<u32>(rtree.rkids.size());
-        return v;
+    RetainView rview() { return image ? dev_rview : retain_view(rtree, rtree.rkids.data(), rtree.redges.data(), rtree.rvals.data()); }
+
+    // one match through engine.cu's launch sequence, its scratch allocated by the plan; returns the control block
+    Ctrl match(const MatchIO& io, bool bulk) {
+        const TrieView tv = view();
+        MatchKnobs kn;
+        kn.tok_bulk = bulk; kn.site_bits = site_bits; kn.pool_rows = pool_rows;
+        const MatchPlan p = plan_match(static_cast<u32>(io.n), tv.max_depth, kn, EMU_SMS, io.hdr != nullptr);
+        Arena a;
+        MatchScratch m{};
+        m.tok = a.get<u32>(p.tok); m.tok8 = a.get<u32>(p.tok8); m.meta = a.get<u32>(p.meta); m.slow = a.get<u32>(p.slow); m.sort = a.get<u32>(p.sort);
+        m.hist = a.get<u32>(p.hist); m.ctrl = a.get<Ctrl>(p.ctrl); m.gstack = a.get<u64>(p.gstack); m.gpool = a.get<Desc>(p.gpool);
+        launch_match(p, m, io, kn, tv, nullptr);
+        return *m.ctrl;
     }
 };
 
@@ -156,7 +170,7 @@ int32_t emu_compact(void* h) {           // gm_compact: dictionary + value compa
     e->trie.compact(&keep, &remap);
     e->rtree.remap_tokens(remap);
     e->i_ranges.up = e->i_values.up = e->i_pool.up = 0; e->up_values_epoch = e->trie.values_epoch;
-    e->i_edges.have = e->i_dict.have = false;
+    e->i_edges.up = e->i_dict.up = 0;
     return 0;
 }
 
@@ -197,86 +211,39 @@ uint64_t emu_retain_bulk_load(void* h, const char* blob, const uint32_t* offs, c
 int32_t emu_match_ex(void* h, const char* blob_in, const uint32_t* offs, uint64_t n_entries, const uint32_t* sel, uint64_t n64, const uint32_t* trees, uint32_t flags,
                      gm_span* out_spans, uint32_t* out_ids, uint64_t cap_ids, uint64_t* needed, int32_t* status, uint64_t* work, uint32_t* deferred) {
     EmuEngine& e = *static_cast<EmuEngine*>(h);
-    const bool desc = flags & 1u, bulk = flags & 2u, stats = flags & 4u, graph_form = flags & 16u;
+    const bool desc = flags & 1u, graph_form = flags & 16u;
     if (!(flags & 8u)) sel = nullptr;
     const u32 n_real = static_cast<u32>(n64);
     *needed = 0;
     if (n_real == 0) return 0;
     if (!e.prepare(false)) return -7;
-    const TrieView tv = e.view();
-    const u32 blob_bytes = offs[n_entries];
+    const Text text(blob_in, offs[n_entries]);
     const u32 n = graph_form ? n_real + 37u : n_real;            // launch size (rows beyond the real batch must stay untouched)
-    u32 hdr_store[4] = {n_real, blob_bytes, 0u, 0u};
-    const u32* hdr = graph_form ? hdr_store : nullptr;
+    const u32 hdr[4] = {n_real, text.bytes, 0u, 0u};
     std::vector<u32> offs_cap;
     if (graph_form) {                                             // the in-block holds capacity + 1 offsets; the tail is never read
         offs_cap.assign(offs, offs + n_entries + 1);
         offs_cap.resize(static_cast<size_t>(n) + 1, 0xDEADBEEFu);
         offs = offs_cap.data();
     }
-    // the bulk stage wants a 16-byte aligned blob that may be read up to a 16-byte boundary
-    const size_t readable = (static_cast<size_t>(blob_bytes) + 15) & ~size_t(15);
-    std::vector<u8> blob_store(readable + 64, 0);
-    u8* blob = blob_store.data() + ((16 - (reinterpret_cast<uintptr_t>(blob_store.data()) & 15)) & 15);
-    std::memcpy(blob, blob_in, blob_bytes);
-    const u32 S = std::max<u32>(1u, tv.max_depth);
-    std::vector<u32> tok(S > TOK8 ? static_cast<size_t>(S) * n : 64), meta(n), slow(n);
-    std::vector<u32> tok8_store(static_cast<size_t>(n) * TOK8 + 16), sort_store(static_cast<size_t>(n) * 11 + 64);
-    u32* tok8 = tok8_store.data() + ((32 - (reinterpret_cast<uintptr_t>(tok8_store.data()) & 31)) & 31) / 4;
-    u32* sortb = sort_store.data() + ((32 - (reinterpret_cast<uintptr_t>(sort_store.data()) & 31)) & 31) / 4;
-    Ctrl ctrl{};
-    const u32 NB = 1u << e.site_bits;
-    std::vector<u32> hist_store(2 * static_cast<size_t>(NB) + 16, 0);
-    u32* hist = hist_store.data() + ((16 - (reinterpret_cast<uintptr_t>(hist_store.data()) & 15)) & 15) / 4;
-    u32* bcursor = hist + NB;
-    u32* bkey = sortb; u32* perm = bkey + n; u32* meta_sorted = perm + n;
-    u32* tok8_sorted = meta_sorted + n + ((8 - (3 * static_cast<size_t>(n)) % 8) % 8);
-    const u32 stack_cap = 32u * (tv.max_depth + 2u) + 64u;
-    const int k3_blocks = EMU_SMS * 4;
-    std::vector<u64> gstack(static_cast<size_t>(k3_blocks) * 8 * stack_cap);
-    const int k2_grid = EMU_SMS * K2_CTAS_PER_SM;
-    std::vector<Desc> gpool(static_cast<size_t>(k2_grid) * K2_THREADS * std::max<u32>(e.pool_rows, 1u));
     std::vector<uint2> descs;
-    std::vector<u32> ids_tmp;
-    void* d_out = out_ids;
-    u64 cap = cap_ids;
-    if (desc) { descs.resize(cap_ids + 1); d_out = descs.data(); }
-
+    if (desc) descs.resize(cap_ids + 1);
     std::vector<int32_t> status_cap;
-    int32_t* status_k = status;
-    if (graph_form) { status_cap.assign(n, 0x7F7F7F7F); status_k = status_cap.data(); }
+    std::vector<gm_span> spans_cap;
     for (u32 i = 0; i < n_real; ++i) status[i] = 0x7F7F7F7F;   // every row must be written by the tokeniser
-    emu::launch(dim3((n + TOK_THREADS - 1) / TOK_THREADS), dim3(TOK_THREADS), [&] {
-        if (bulk) k_tokenize<true>(blob, blob_bytes, static_cast<u32>(readable), offs, sel, n, hdr, tv, S, tok8, tok.data(), meta.data(), status_k, bkey, hist, e.site_bits, 0u);
-        else k_tokenize<false>(blob, blob_bytes, static_cast<u32>(readable), offs, sel, n, hdr, tv, S, tok8, tok.data(), meta.data(), status_k, bkey, hist, e.site_bits, 0u);
-    });
-    emu::launch(dim3(1), dim3(1024), [&] { k_bucket_scan(hist, bcursor, NB); });
-    emu::launch(dim3((n + 255) / 256), dim3(256), [&] { k_bucket_scatter(bkey, bcursor, n, hdr, perm, tok8, meta.data(), tok8_sorted, meta_sorted); });
+    if (graph_form) { status_cap.assign(n, 0x7F7F7F7F); spans_cap.assign(n, gm_span{0xABABABABu, 0xABABABABu}); }
+
+    MatchIO io;
+    io.blob = text.p; io.blob_bytes = text.bytes; io.readable_bytes = text.readable; io.offs = offs; io.sel = sel; io.n = n; io.trees = trees;
+    io.hdr = graph_form ? hdr : nullptr;
+    io.spans = graph_form ? spans_cap.data() : out_spans; io.status = graph_form ? status_cap.data() : status;
+    io.out = desc ? static_cast<void*>(descs.data()) : out_ids; io.cap = cap_ids;
+    io.stats = flags & 4u; io.desc = desc;
+    const Ctrl ctrl = e.match(io, flags & 2u);
     if (graph_form) {
         for (u32 i = n_real; i < n; ++i) if (status_cap[i] != 0x7F7F7F7F) return -50;      // a row beyond the real batch was touched
-        std::memcpy(status, status_cap.data(), n_real * sizeof(int32_t));
-    }
-    std::vector<gm_span> spans_cap;
-    gm_span* spans_k = out_spans;
-    if (graph_form) { spans_cap.assign(n, gm_span{0xABABABABu, 0xABABABABu}); spans_k = spans_cap.data(); }
-
-    MatchParams mp{};
-    mp.tv = tv; mp.tok8 = tok8; mp.tok = tok.data(); mp.meta = meta.data(); mp.n = n; mp.n_ptr = hdr; mp.tok_levels = S;
-    mp.spans = reinterpret_cast<uint2*>(spans_k); mp.out_ids = static_cast<u32*>(d_out); mp.out_desc = static_cast<uint2*>(d_out); mp.cap_ids = cap;
-    mp.status = status_k; mp.trees = trees;
-    mp.cursor = &ctrl.cursor; mp.slow_list = slow.data(); mp.slow_count = &ctrl.slow_count; mp.tile_counter = &ctrl.tile_counter; mp.stats = ctrl.stats;
-    mp.perm = perm; mp.tok8_sorted = tok8_sorted; mp.meta_sorted = meta_sorted;
-    mp.flags = MP_SORTED_ROWS; mp.tile_chunk = 1;
-    emu::launch(dim3(k2_grid), dim3(K2_THREADS), [&] {
-        if (stats) { if (desc) k_match_fast<K2_FAST_L, K2_THREADS, K2_CTAS_PER_SM, true, true>(mp, gpool.data(), e.pool_rows); else k_match_fast<K2_FAST_L, K2_THREADS, K2_CTAS_PER_SM, true, false>(mp, gpool.data(), e.pool_rows); }
-        else { if (desc) k_match_fast<K2_FAST_L, K2_THREADS, K2_CTAS_PER_SM, false, true>(mp, gpool.data(), e.pool_rows); else k_match_fast<K2_FAST_L, K2_THREADS, K2_CTAS_PER_SM, false, false>(mp, gpool.data(), e.pool_rows); }
-    });
-    emu::launch(dim3(k3_blocks), dim3(256), [&] {
-        if (stats) { if (desc) k_match_slow<true, true>(mp, gstack.data(), stack_cap); else k_match_slow<true, false>(mp, gstack.data(), stack_cap); }
-        else { if (desc) k_match_slow<false, true>(mp, gstack.data(), stack_cap); else k_match_slow<false, false>(mp, gstack.data(), stack_cap); }
-    });
-    if (graph_form) {
         for (u32 i = n_real; i < n; ++i) if (spans_cap[i].off != 0xABABABABu) return -51;
+        std::memcpy(status, status_cap.data(), n_real * sizeof(int32_t));
         std::memcpy(out_spans, spans_cap.data(), n_real * sizeof(gm_span));
     }
     if (deferred) *deferred = ctrl.slow_count;
@@ -285,6 +252,7 @@ int32_t emu_match_ex(void* h, const char* blob_in, const uint32_t* offs, uint64_
     if (ctrl.cursor > cap_ids) return -3;
     if (!desc) return 0;
     // descriptor mode: expand (ref, cnt) into ids out of the host mirror, per topic, so that the caller compares id lists
+    std::vector<u32> ids_tmp;
     u64 w = 0;
     for (u32 t = 0; t < n_real; ++t) {
         const u32 off = out_spans[t].off, cnt = out_spans[t].cnt;
@@ -324,25 +292,15 @@ int32_t emu_partition(const char* blob, const uint32_t* offs, uint64_t n, uint32
 }
 
 // ---- the fused gather over "peer memory": every rank's block lives in host memory of this one process ---------------------------
-struct GatherWorld {
-    u32 world = 0; u64 slab_topics = 0, slab_ids = 0;
-    static constexpr size_t off_ids = 256;
-    size_t off_spans = 0, off_index = 0, off_counts = 0, off_flags = 0, bytes = 0;
+struct GatherWorld : GatherLayout {
     std::vector<std::vector<char>> store;
     std::vector<char*> block;
     std::vector<u32> epoch;
     std::vector<unsigned long long> cursor;      // the match cursor of every rank's last step (k_gather_push / k_gather_finish read it)
 };
-void* emu_gather_new(uint32_t world, uint64_t slab_topics, uint64_t slab_ids) {       // engine.cu gm_gather_create's layout
+void* emu_gather_new(uint32_t world, uint64_t slab_topics, uint64_t slab_ids) {
     GatherWorld* g = new GatherWorld();
-    slab_topics = (slab_topics + 3) & ~uint64_t(3); slab_ids = (slab_ids + 3) & ~uint64_t(3);
-    g->world = world; g->slab_topics = slab_topics; g->slab_ids = slab_ids;
-    const size_t a = 256;
-    g->off_spans = (GatherWorld::off_ids + static_cast<size_t>(world) * slab_ids * 4 + a - 1) / a * a;
-    g->off_index = g->off_spans + static_cast<size_t>(world) * slab_topics * 8;
-    g->off_counts = (g->off_index + static_cast<size_t>(world) * slab_topics * 4 + a - 1) / a * a;
-    g->off_flags = g->off_counts + static_cast<size_t>(world) * 16;
-    g->bytes = g->off_flags + 256;
+    static_cast<GatherLayout&>(*g) = gather_layout(world, slab_topics, slab_ids);
     g->store.resize(world); g->block.resize(world); g->epoch.assign(world, 0); g->cursor.assign(world, 0);
     for (u32 w = 0; w < world; ++w) {
         g->store[w].assign(g->bytes + 256, static_cast<char>(0xEE));        // (stale bytes must never be read as results)
@@ -366,59 +324,17 @@ int32_t emu_match_gather(void* gw, uint32_t rank, void* h, const char* blob_in, 
     G.cursor[rank] = 0;
     if (n) {
         if (!e.prepare(false)) return -7;
-        const TrieView tv = e.view();
-        const u32 blob_bytes = offs[n_entries];
-        const size_t readable = (static_cast<size_t>(blob_bytes) + 15) & ~size_t(15);
-        std::vector<u8> blob_store(readable + 64, 0);
-        u8* blob = blob_store.data() + ((16 - (reinterpret_cast<uintptr_t>(blob_store.data()) & 15)) & 15);
-        std::memcpy(blob, blob_in, blob_bytes);
-        const u32 S = std::max<u32>(1u, tv.max_depth);
-        std::vector<u32> tok(S > TOK8 ? static_cast<size_t>(S) * n : 64), meta(n), slow(n);
-        std::vector<u32> tok8_store(static_cast<size_t>(n) * TOK8 + 16), sort_store(static_cast<size_t>(n) * 11 + 64);
-        u32* tok8 = tok8_store.data() + ((32 - (reinterpret_cast<uintptr_t>(tok8_store.data()) & 31)) & 31) / 4;
-        u32* sortb = sort_store.data() + ((32 - (reinterpret_cast<uintptr_t>(sort_store.data()) & 31)) & 31) / 4;
-        Ctrl ctrl{};
-        const u32 NB = 1u << e.site_bits;
-        std::vector<u32> hist_store(2 * static_cast<size_t>(NB) + 16, 0);
-        u32* hist = hist_store.data() + ((16 - (reinterpret_cast<uintptr_t>(hist_store.data()) & 15)) & 15) / 4;
-        u32* bcursor = hist + NB;
-        u32* bkey = sortb; u32* perm = bkey + n; u32* meta_sorted = perm + n;
-        u32* tok8_sorted = meta_sorted + n + ((8 - (3 * static_cast<size_t>(n)) % 8) % 8);
-        const u32 stack_cap = 32u * (tv.max_depth + 2u) + 64u;
-        const int k3_blocks = EMU_SMS * 4, k2_grid = EMU_SMS * K2_CTAS_PER_SM;
-        std::vector<u64> gstack(static_cast<size_t>(k3_blocks) * 8 * stack_cap);
-        std::vector<Desc> gpool(static_cast<size_t>(k2_grid) * K2_THREADS * std::max<u32>(e.pool_rows, 1u));
-        emu::launch(dim3((n + TOK_THREADS - 1) / TOK_THREADS), dim3(TOK_THREADS), [&] {
-            k_tokenize<false>(blob, blob_bytes, static_cast<u32>(readable), offs, sel, n, nullptr, tv, S, tok8, tok.data(), meta.data(), status, bkey, hist, e.site_bits, 0u);
-        });
-        emu::launch(dim3(1), dim3(1024), [&] { k_bucket_scan(hist, bcursor, NB); });
-        emu::launch(dim3((n + 255) / 256), dim3(256), [&] { k_bucket_scatter(bkey, bcursor, n, nullptr, perm, tok8, meta.data(), tok8_sorted, meta_sorted); });
-        MatchParams mp{};
-        mp.tv = tv; mp.tok8 = tok8; mp.tok = tok.data(); mp.meta = meta.data(); mp.n = n; mp.tok_levels = S;
-        mp.cap_ids = G.slab_ids; mp.status = status;
-        mp.cursor = &ctrl.cursor; mp.slow_list = slow.data(); mp.slow_count = &ctrl.slow_count; mp.tile_counter = &ctrl.tile_counter; mp.stats = ctrl.stats;
-        mp.perm = perm; mp.tok8_sorted = tok8_sorted; mp.meta_sorted = meta_sorted;
-        mp.flags = MP_SORTED_ROWS; mp.tile_chunk = 1;
-        mp.g_base_topics = static_cast<u32>(rank * G.slab_topics); mp.g_base_ids = rank * G.slab_ids; mp.g_sel = sel;     // engine.cu enqueue_match, gather_mode
-        if (direct) {
-            mp.g_world = G.world;
-            for (u32 w = 0; w < G.world; ++w) {
-                mp.g_ids[w] = reinterpret_cast<u32*>(G.block[w] + GatherWorld::off_ids); mp.g_spans[w] = reinterpret_cast<uint2*>(G.block[w] + G.off_spans);
-                mp.g_index[w] = reinterpret_cast<u32*>(G.block[w] + G.off_index);
-            }
-        } else {
-            mp.g_world = 1;
-            mp.g_ids[0] = reinterpret_cast<u32*>(G.block[rank] + GatherWorld::off_ids); mp.g_spans[0] = reinterpret_cast<uint2*>(G.block[rank] + G.off_spans);
-            mp.g_index[0] = reinterpret_cast<u32*>(G.block[rank] + G.off_index);
-        }
-        emu::launch(dim3(k2_grid), dim3(K2_THREADS), [&] { k_match_fast<K2_FAST_L, K2_THREADS, K2_CTAS_PER_SM, false, false, true>(mp, gpool.data(), e.pool_rows); });
-        emu::launch(dim3(k3_blocks), dim3(256), [&] { k_match_slow<false, false, true>(mp, gstack.data(), stack_cap); });
-        G.cursor[rank] = ctrl.cursor;
-        if (ctrl.cursor > G.slab_ids) return -3;
+        const Text text(blob_in, offs[n_entries]);
+        const GatherTarget target{&G, G.block.data(), rank, direct != 0};
+        MatchIO io;
+        io.blob = text.p; io.blob_bytes = text.bytes; io.readable_bytes = text.readable; io.offs = offs; io.sel = sel; io.n = n;
+        io.cap = G.slab_ids; io.status = status; io.gather = &target;
+        G.cursor[rank] = e.match(io, false).cursor;
+        if (G.cursor[rank] > G.slab_ids) return -3;
     }
     if (!direct && G.world > 1)
         emu::launch(dim3(EMU_SMS * 4), dim3(256), [&] {
-            k_gather_push(G.block.data(), rank, G.world, GatherWorld::off_ids, G.off_spans, G.off_index, rank * G.slab_topics, rank * G.slab_ids, n, &G.cursor[rank]);
+            k_gather_push(G.block.data(), rank, G.world, GatherLayout::off_ids, G.off_spans, G.off_index, rank * G.slab_topics, rank * G.slab_ids, n, &G.cursor[rank]);
         });
     return 0;
 }
@@ -443,7 +359,7 @@ void emu_gather_read(void* gw, uint32_t rank, uint64_t* counts, uint32_t* index,
     std::memcpy(counts, b + G.off_counts, static_cast<size_t>(G.world) * 16);
     std::memcpy(index, b + G.off_index, static_cast<size_t>(G.world) * G.slab_topics * 4);
     std::memcpy(spans, b + G.off_spans, static_cast<size_t>(G.world) * G.slab_topics * 8);
-    std::memcpy(ids, b + GatherWorld::off_ids, static_cast<size_t>(G.world) * G.slab_ids * 4);
+    std::memcpy(ids, b + GatherLayout::off_ids, static_cast<size_t>(G.world) * G.slab_ids * 4);
 }
 
 // RetainStorage::get for a batch of filters through k_tokenize -> k_retain_init -> k_retain_round x (depth + 1) -> k_retain_scan -> k_retain_expand
@@ -456,44 +372,19 @@ int32_t emu_retain_match(void* h, const char* blob_in, const uint32_t* offs, uin
     if (!e.prepare(true)) return -7;
     const TrieView tv = e.view();
     const RetainView rv = e.rview();
-    const u32 depth = rv.max_depth, S = depth + 2;
-    const u32 blob_bytes = offs[nq];
-    std::vector<u8> blob_store(static_cast<size_t>(blob_bytes) + 64, 0);
-    u8* blob = blob_store.data() + ((16 - (reinterpret_cast<uintptr_t>(blob_store.data()) & 15)) & 15);
-    std::memcpy(blob, blob_in, blob_bytes);
-    std::vector<u32> tok(S > TOK8 ? static_cast<size_t>(S) * nq : 64), meta(nq);
-    std::vector<u32> tok8_store(static_cast<size_t>(nq) * TOK8 + 16);
-    u32* tok8 = tok8_store.data() + ((32 - (reinterpret_cast<uintptr_t>(tok8_store.data()) & 31)) & 31) / 4;
-    struct RCtl { unsigned long long grand; unsigned long long stats[2]; u32 err; u32 pad; u32 n_desc[RQ]; };
-    RCtl ctl{};
-    std::vector<u32> counts(static_cast<size_t>(depth + 3) * RQ + (depth + 3), 0);
-    std::vector<u32> rq(static_cast<size_t>(nq) * 3, 0);
-    u32* qtotal = rq.data(); u32* qbase = qtotal + nq; u32* qcur = qbase + nq;
-    const u32 slice_items = std::max<u32>(1u, cap_items / RQ), slice_desc = std::max<u32>(1u, cap_desc / RQ);
-    std::vector<RTask> front[2] = {std::vector<RTask>(static_cast<size_t>(slice_items) * RQ), std::vector<RTask>(static_cast<size_t>(slice_items) * RQ)};
-    std::vector<RDesc> rdescs(static_cast<size_t>(slice_desc) * RQ);
+    const Text text(blob_in, offs[nq]);
+    const RetainPlan p = plan_retain(nq, rv.max_depth, cap_items, cap_desc, EMU_SMS);
+    Arena a;
+    RetainScratch r{};
+    r.tok = a.get<u32>(p.tok); r.tok8 = a.get<u32>(p.tok8); r.meta = a.get<u32>(p.meta); r.rq = a.get<u32>(p.rq); r.ctl = a.get<RCtl>(p.ctl);
+    r.front[0] = a.get<RTask>(p.front); r.front[1] = a.get<RTask>(p.front); r.descs = a.get<RDesc>(p.descs);
     for (u32 i = 0; i < nq; ++i) status[i] = 0x7F7F7F7F;
-    emu::launch(dim3((nq + TOK_THREADS - 1) / TOK_THREADS), dim3(TOK_THREADS), [&] {
-        k_tokenize<false>(blob, blob_bytes, blob_bytes, offs, nullptr, nq, nullptr, tv, S, tok8, tok.data(), meta.data(), status, nullptr, nullptr, 0u, 0u);
-    });
-    RetainParams rp{};
-    rp.v = rv; rp.qtok8 = tok8; rp.qtok = tok.data(); rp.qmeta = meta.data(); rp.nq = nq; rp.tok_levels = S;
-    rp.descs = rdescs.data(); rp.n_desc = ctl.n_desc; rp.cap_items = slice_items; rp.cap_desc = slice_desc;
-    rp.qtotal = qtotal; rp.err = &ctl.err; rp.stats = ctl.stats;
-    emu::launch(dim3((nq + 255) / 256), dim3(256), [&] { if (stats_on) k_retain_init<true>(rp, front[0].data(), &counts[0]); else k_retain_init<false>(rp, front[0].data(), &counts[0]); });
-    const int rgrid = EMU_SMS * GM_RETAIN_CTAS;
-    for (u32 lvl = 0; lvl <= depth; ++lvl)
-        emu::launch(dim3(rgrid), dim3(256), [&] {
-            u32* claim = &counts[static_cast<size_t>(depth + 3) * RQ + lvl];
-            if (stats_on) k_retain_round<true>(rp, front[lvl & 1].data(), &counts[static_cast<size_t>(lvl) * RQ], front[(lvl + 1) & 1].data(), &counts[static_cast<size_t>(lvl + 1) * RQ], claim);
-            else k_retain_round<false>(rp, front[lvl & 1].data(), &counts[static_cast<size_t>(lvl) * RQ], front[(lvl + 1) & 1].data(), &counts[static_cast<size_t>(lvl + 1) * RQ], claim);
-        });
-    emu::launch(dim3(1), dim3(1024), [&] { k_retain_scan(qtotal, nq, qbase, reinterpret_cast<uint2*>(out_spans), &ctl.grand); });
-    emu::launch(dim3(EMU_SMS * 8), dim3(256), [&] { k_retain_expand(rdescs.data(), ctl.n_desc, slice_desc, rv.vals, qbase, qcur, out_ids, cap_ids); });
+    launch_retain(p, r, tv, rv, text.p, text.bytes, offs, out_spans, out_ids, cap_ids, status, stats_on != 0, nullptr);
+    RCtl& ctl = *r.ctl;
     if (work) { work[0] = ctl.stats[0]; work[1] = ctl.stats[1]; }
     if (ctl.err) return -100 - static_cast<int32_t>(ctl.err);      // scratch overflow: bit 0 tasks, bit 1 descriptors (the engine grows and retries)
-    e.last_tasks.assign(depth + 2, 0);                             // the totals of engine.cu's `retain stats` line
-    for (u32 l = 0; l <= depth + 1; ++l) for (u32 k = 0; k < RQ; ++k) e.last_tasks[l] += counts[static_cast<size_t>(l) * RQ + k];
+    e.last_tasks.assign(p.depth + 2, 0);                           // the totals of engine.cu's `retain stats` line
+    for (u32 l = 0; l <= p.depth + 1; ++l) for (u32 k = 0; k < RQ; ++k) e.last_tasks[l] += ctl.round_counts(l)[k];
     e.last_n_desc = 0;
     for (u32 k = 0; k < RQ; ++k) e.last_n_desc += ctl.n_desc[k];
     *needed = ctl.grand;

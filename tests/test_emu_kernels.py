@@ -1,6 +1,6 @@
 """CPU tier: the REAL kernel sources (rmqtt_b200/csrc/kernels.cuh, retain_kernels.cuh, relations.cuh) executed on the CPU by
 the small CUDA-model emulation under tests/native/emu (threads of a CTA as fibers, warp collectives and barriers as
-rendezvous points), driven like engine.cu drives them, and compared with the oracle — bit-exact sorted multisets, plus the
+rendezvous points), driven by engine.cu's own launch code (pipeline.cuh), and compared with the oracle — bit-exact sorted multisets, plus the
 exact work counters V / E / F / M of the instrumented instantiations.
 
 What this tier adds to the GPU tier: it runs HERE (no device), so a logic or indexing regression in a kernel shows up in the
