@@ -223,7 +223,8 @@ typedef struct gm_sub_opts {      /* rmqtt::types::SubscriptionOptions (types.rs
 typedef struct gm_sub_relation {  /* one element of SubRelations (types.rs:445-453) */
     uint64_t node_id;
     uint32_t handle;              /* -> (topic_filter, client_id) through gmr_relation */
-    uint32_t group;               /* 0, or the id of the (filter, shared group) this member belongs to: the caller chooses one member */
+    uint32_t group;               /* 0, or the id of the (filter, shared group) this member belongs to: gmr_matches_batch returns every
+                                     member (the caller chooses), gmr_matches_batch_shared the chosen one (| GM_SUBREL_OFFLINE) */
     uint32_t sub_ids_off, sub_ids_cnt; /* v5: accumulated subscription identifiers in out_sub_ids */
 } gm_sub_relation;
 int32_t gmr_create(gm_engine* e, gm_router** out);   /* the router uses, but does not own, the engine */
@@ -254,6 +255,25 @@ int32_t gmr_matched_filters_batch(gm_router* r, const char* topics_blob, const u
 int32_t gmr_filter(gm_router* r, uint32_t filter_idx, const char** filter, uint32_t* filter_len, uint64_t* out_node_ids, uint32_t cap_nodes,
                    uint32_t* n_nodes);
 int32_t gmr_relation(gm_router* r, uint32_t handle, const char** filter, uint32_t* filter_len, const char** client, uint32_t* client_len);
+/* ---- shared subscriptions chosen on the device (gm_relations_choose_device): with these calls gmr_matches_batch_shared IS
+ *      Router::matches — ONE member per matched (filter, group), preferring online clients.  So that a caller can reproduce the
+ *      draw, the router numbers as follows, and never reuses a number:
+ *        group ids   1, 2, ... in order of the first successful gmr_add of each (filter, shared group);
+ *        client keys 0, 1, ... in order of the first successful gmr_add (or gmr_add_batch_numbered) or gmr_set_online that names
+ *                    each (node_id, client_id).
+ *      Row = the topic's index in the call.                                                                                       */
+/* Router::is_online as the router knows it: a client it has never been told about is online. */
+int32_t gmr_set_online(gm_router* r, uint64_t node_id, const char* client, uint32_t len, int32_t online);
+/* gmr_matches_batch with the choice: a chosen record's `group` is its group id | GM_SUBREL_OFFLINE when no eligible member was
+ * online; chosen v5 members are de-duplicated per client with the topic's other v5 relations.  gmr_matches_batch itself keeps
+ * returning every member.                                                                                                      */
+int32_t gmr_matches_batch_shared(gm_router* r, uint64_t seed, const gm_id* publishers, const char* topics_blob, const uint32_t* topic_offsets,
+                                 uint64_t n, gm_span* out_spans, gm_sub_relation* out_rels, uint64_t cap_rels, uint32_t* out_sub_ids,
+                                 uint64_t cap_sub_ids, uint64_t* needed_rels, uint64_t* needed_sub_ids, int32_t* status);
+/* a group's filter, name and current member handles (the group_cids of SharedGroupType); *n = the member count, at most cap of them
+ * are written.  GM_ERR_INVALID_ARG for an unknown group id.                                                                        */
+int32_t gmr_group(gm_router* r, uint32_t group, const char** filter, uint32_t* flen, const char** name, uint32_t* nlen, uint32_t* out_handles,
+                  uint32_t cap, uint32_t* n);
 
 /* ---- single-call front end: Router::matches is called once per PUBLISH from many tokio workers (rmqtt/src/router.rs:482-484,
  *      caller rmqtt/src/shared.rs:601-636).  The batcher turns single submissions into device batches: a mutex-protected
@@ -343,6 +363,34 @@ typedef struct gm_rel_out {
  * (NULL: no no_local filtering); d_rels[n_rels]: the relation table.  Asynchronous on `stream`.                                   */
 int32_t gm_relations_expand_device(gm_engine* e, const gm_span* d_spans, const uint32_t* d_ids, uint64_t n, const uint32_t* d_publishers,
                                    const gm_rel* d_rels, uint64_t n_rels, const gm_rel_out* out, void* stream);
+/* The same expansion with the shared-subscription choice (rmqtt/src/router.rs:192-238, rmqtt/src/subscribe.rs:66-104) made on the
+ * device: per matched (filter, group) ONE member.  The draw is a random-key minimum: every eligible member (live, not dropped by
+ * no_local) gets key = gm_share_key(seed, row, group, occ, client_key), where row is the topic's index in the call and occ = 0 .. m-1
+ * numbers the m appearances of the group's filter node in the row (a topic with a literal '+' / '#' level matches a wildcard node
+ * twice).  The chosen member is the eligible ONLINE member with the smallest (key, client_key); if none is online, the smallest of
+ * all eligible members, flagged offline; without eligible members nothing is chosen.  That is uniform over the online members,
+ * otherwise over all of them, like the reference's random choice, and reproducible from the seed.
+ * The group table: d_groups[g] = {off, cnt} locates group g's member handles in d_members (any order).  In the match list a
+ * shared relation triggers the choice only if it is its group's representative d_members[d_groups[g].off]; every other member
+ * entry is dropped, and so is a relation whose group id is >= n_groups or whose block is empty.  A chosen v3 member is a record of
+ * its own; a chosen v5 member is de-duplicated per client with the row's other v5 relations (a merged record carries the handle
+ * and group field of the client's smallest handle).  A chosen record's `group` is the group id, | GM_SUBREL_OFFLINE when it was
+ * chosen offline: the (group, is_online) of the reference's SharedGroupType.  Same arguments, checks and capacity protocol as
+ * gm_relations_expand_device.                                                                                                     */
+#define GM_SUBREL_OFFLINE 0x80000000u
+typedef struct gm_rel_groups {
+    const gm_span* d_groups; uint32_t n_groups;       /* index = group id; [0] unused */
+    const uint32_t* d_members;
+    const uint32_t* d_online; uint32_t n_online_bits; /* one bit per client_key, 1 = online; NULL: every client online; a key past
+                                                         n_online_bits counts as offline */
+    uint64_t seed;
+} gm_rel_groups;
+int32_t gm_relations_choose_device(gm_engine* e, const gm_span* d_spans, const uint32_t* d_ids, uint64_t n, const uint32_t* d_publishers,
+                                   const gm_rel* d_rels, uint64_t n_rels, const gm_rel_groups* g, const gm_rel_out* out, void* stream);
+/* the key of the draw (pure host function; the kernel uses the same code):
+ *   mix(x) = x ^= x >> 30; x *= 0xbf58476d1ce4e5b9; x ^= x >> 27; x *= 0x94d049bb133111eb; x ^= x >> 31      (u64)
+ *   key    = mix(mix(seed ^ (row << 32 | group)) ^ (occ << 32 | client_key))                                                 */
+uint64_t gm_share_key(uint64_t seed, uint32_t row, uint32_t group, uint32_t occ, uint32_t client_key);
 
 /* ---- the same exchange FUSED into the match kernels over peer memory (NVLink / NVSwitch): the publish phase of the match writes
  *      every topic's span, global index and ids directly into the gathered arrays of ALL ranks while the walk of the next tiles is

@@ -119,6 +119,7 @@ pub const GM_IPC_HANDLE_BYTES: usize = 64;
 pub const GM_REL_LIVE: u32 = 1;
 pub const GM_REL_V5: u32 = 2;
 pub const GM_REL_NO_LOCAL: u32 = 4;
+pub const GM_SUBREL_OFFLINE: u32 = 0x8000_0000;
 
 #[repr(C)]
 #[derive(Clone, Copy, Default, Debug)]
@@ -245,6 +246,15 @@ pub struct gm_rel_out {
     pub d_status: *mut i32,
 }
 #[repr(C)]
+pub struct gm_rel_groups {
+    pub d_groups: *const gm_span,
+    pub n_groups: u32,
+    pub d_members: *const u32,
+    pub d_online: *const u32,
+    pub n_online_bits: u32,
+    pub seed: u64,
+}
+#[repr(C)]
 pub struct gm_gather_view {
     pub d_index: *const u32,
     pub d_spans: *const gm_span,
@@ -288,6 +298,12 @@ extern "C" {
                       n_nodes: *mut u32) -> i32;
     pub fn gmr_relation(r: *mut gm_router, handle: u32, filter: *mut *const c_char, filter_len: *mut u32, client: *mut *const c_char,
                         client_len: *mut u32) -> i32;
+    pub fn gmr_set_online(r: *mut gm_router, node_id: u64, client: *const c_char, len: u32, online: i32) -> i32;
+    pub fn gmr_matches_batch_shared(r: *mut gm_router, seed: u64, publishers: *const gm_id, topics_blob: *const u8, topic_offsets: *const u32,
+                                    n: u64, out_spans: *mut gm_span, out_rels: *mut gm_sub_relation, cap_rels: u64, out_sub_ids: *mut u32,
+                                    cap_sub_ids: u64, needed_rels: *mut u64, needed_sub_ids: *mut u64, status: *mut i32) -> i32;
+    pub fn gmr_group(r: *mut gm_router, group: u32, filter: *mut *const c_char, flen: *mut u32, name: *mut *const c_char, nlen: *mut u32,
+                     out_handles: *mut u32, cap: u32, n: *mut u32) -> i32;
     // wire side + probes
     pub fn gm_publish_topic(packet: *const u8, len: u32, topic: *mut *const c_char, topic_len: *mut u32) -> i32;
     pub fn gm_batcher_probe(e: *mut gm_engine, blob: *const u8, offsets: *const u32, n: u64, burst: u32, rounds: u32, max_wait_us: u32,
@@ -306,6 +322,9 @@ extern "C" {
                                 sizes: *mut u64, stream: *mut c_void) -> i32;
     pub fn gm_relations_expand_device(e: *mut gm_engine, d_spans: *const gm_span, d_ids: *const u32, n: u64, d_publishers: *const u32,
                                       d_rels: *const gm_rel, n_rels: u64, out: *const gm_rel_out, stream: *mut c_void) -> i32;
+    pub fn gm_relations_choose_device(e: *mut gm_engine, d_spans: *const gm_span, d_ids: *const u32, n: u64, d_publishers: *const u32,
+                                      d_rels: *const gm_rel, n_rels: u64, g: *const gm_rel_groups, out: *const gm_rel_out, stream: *mut c_void) -> i32;
+    pub fn gm_share_key(seed: u64, row: u32, group: u32, occ: u32, client_key: u32) -> u64;
     pub fn gm_gather_create(e: *mut gm_engine, world: u32, rank: u32, slab_topics: u64, slab_ids: u64, out_handle: *mut u8) -> i32;
     pub fn gm_gather_connect(e: *mut gm_engine, handles: *const u8) -> i32;
     pub fn gm_match_gather_device(e: *mut gm_engine, d_blob: *const c_void, blob_bytes: u64, d_offsets: *const u32, n_entries: u64,

@@ -53,6 +53,14 @@ class GmSubRelation(C.Structure):
     _fields_ = [("node_id", C.c_uint64), ("handle", C.c_uint32), ("group", C.c_uint32), ("sub_ids_off", C.c_uint32), ("sub_ids_cnt", C.c_uint32)]
 
 
+GM_SUBREL_OFFLINE = 0x80000000
+
+
+class GmRelGroups(C.Structure):
+    _fields_ = [("d_groups", C.c_void_p), ("n_groups", C.c_uint32), ("d_members", C.c_void_p), ("d_online", C.c_void_p),
+                ("n_online_bits", C.c_uint32), ("seed", C.c_uint64)]
+
+
 class GmWork(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("visited", "probed", "filters", "ids", "levels", "bytes", "deferred")] + \
                [("probes_by_depth", C.c_uint64 * 8), ("misses_by_depth", C.c_uint64 * 8), ("slot_loads", C.c_uint64)]
@@ -134,6 +142,8 @@ SIGNATURES = {
     "gm_batcher_probe": (_i32, [_vp, _vp, _vp, _u64, _u32, _u32, _u32, _P(GmLatency)]),
     "gm_churn_probe": (_i32, [_vp, _vp, _vp, _vp, _u64, C.c_double, _u32, _u32, _P(GmChurn)]),
     "gm_relations_expand_device": (_i32, [_vp, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _vp]),
+    "gm_relations_choose_device": (_i32, [_vp, _vp, _vp, _u64, _vp, _vp, _u64, _P(GmRelGroups), _vp, _vp]),
+    "gm_share_key": (_u64, [_u64, _u32, _u32, _u32, _u32]),
     "gm_gather_create": (_i32, [_vp, _u32, _u32, _u64, _u64, _vp]),
     "gm_gather_connect": (_i32, [_vp, _vp]),
     "gm_match_gather_device": (_i32, [_vp, _vp, _u64, _vp, _u64, _vp, _u64, _vp, _vp]),
@@ -163,6 +173,9 @@ SIGNATURES = {
     "gmr_matched_filters_batch": (_i32, [_vp, _vp, _vp, _u64, _vp, _vp, _u64, _P(_u64), _vp]),
     "gmr_filter": (_i32, [_vp, _u32, _P(_cp), _P(_u32), _vp, _u32, _P(_u32)]),
     "gmr_relation": (_i32, [_vp, _u32, _P(_cp), _P(_u32), _P(_cp), _P(_u32)]),
+    "gmr_set_online": (_i32, [_vp, _u64, _cp, _u32, _i32]),
+    "gmr_matches_batch_shared": (_i32, [_vp, _u64, _vp, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _u64, _P(_u64), _P(_u64), _vp]),
+    "gmr_group": (_i32, [_vp, _u32, _P(_cp), _P(_u32), _P(_cp), _P(_u32), _vp, _u32, _P(_u32)]),
     "gm_tokenize_batch": (_i32, [_vp, _vp, _vp, _u64, _u32, _vp, _vp]),
     "gm_get_stats": (_i32, [_vp, _P(GmStats)]),
     "gm_kernel_ms_ring": (_i32, [_vp, _vp, _u32, _P(_u32)]),

@@ -1154,6 +1154,36 @@ int32_t gmr_matches_batch(gm_router* r, const gm_id* publishers, const char* blo
     return rc;
 }
 
+int32_t gmr_matches_batch_shared(gm_router* r, uint64_t seed, const gm_id* publishers, const char* blob, const uint32_t* offs, uint64_t n, gm_span* out_spans,
+                                 gm_sub_relation* out_rels, uint64_t cap_rels, uint32_t* out_sub_ids, uint64_t cap_sub_ids, uint64_t* needed_rels,
+                                 uint64_t* needed_sub_ids, int32_t* status) {
+    if (!r || (n && (!offs || !out_spans || !status))) return GM_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> g(r->impl.mu);
+    const int32_t rc = r->impl.matches_batch(publishers, blob, offs, n, out_spans, out_rels, cap_rels, out_sub_ids, cap_sub_ids, needed_rels, needed_sub_ids, status, &seed);
+    if (rc == GM_ERR_CAPACITY) g_err = "gmr_matches_batch_shared: output too small";
+    return rc;
+}
+
+int32_t gmr_set_online(gm_router* r, uint64_t node_id, const char* client, uint32_t len, int32_t online) {
+    if (!r || (!client && len)) return GM_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> g(r->impl.mu);
+    r->impl.set_online(node_id, client ? std::string(client, len) : std::string(), online != 0);
+    return GM_OK;
+}
+
+int32_t gmr_group(gm_router* r, uint32_t group, const char** filter, uint32_t* flen, const char** name, uint32_t* nlen, uint32_t* out_handles, uint32_t cap, uint32_t* n) {
+    if (!r || !filter || !flen || !name || !nlen) return GM_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> g(r->impl.mu);
+    const std::string *f, *gn;
+    const uint32_t* members;
+    uint32_t cnt = 0;
+    if (!r->impl.group(group, &f, &gn, &members, &cnt)) return GM_ERR_INVALID_ARG;
+    *filter = f->data(); *flen = static_cast<uint32_t>(f->size()); *name = gn->data(); *nlen = static_cast<uint32_t>(gn->size());
+    if (n) *n = cnt;
+    if (out_handles) std::copy(members, members + std::min(cnt, cap), out_handles);
+    return GM_OK;
+}
+
 int32_t gmr_matched_filters_batch(gm_router* r, const char* blob, const uint32_t* offs, uint64_t n, gm_span* out_spans, uint32_t* out_filters, uint64_t cap_filters,
                                   uint64_t* needed, int32_t* status) {
     if (!r || (n && (!offs || !out_spans || !status))) return GM_ERR_INVALID_ARG;
@@ -1475,6 +1505,34 @@ int32_t gm_relations_expand_device(gm_engine* e, const gm_span* d_spans, const u
     CUDA_TRY(cudaGetLastError());
     return GM_OK;
 }
+
+int32_t gm_relations_choose_device(gm_engine* e, const gm_span* d_spans, const uint32_t* d_ids, uint64_t n, const uint32_t* d_publishers,
+                                   const gm_rel* d_rels, uint64_t n_rels, const gm_rel_groups* gr, const gm_rel_out* o, void* stream) {
+    if (!e || !o || !gr || !o->d_needed || (n && (!d_spans || !o->d_spans || !o->d_status)) || (gr->n_groups && (!gr->d_groups || !gr->d_members)))
+        return GM_ERR_INVALID_ARG;
+    if (n > 0xFFFFFFF0ull || n_rels > 0xFFFFFFFFull) { g_err = "batch too large"; return GM_ERR_TOO_LARGE; }
+    if (e->flags & GM_FLAG_HOST_ONLY) { g_err = "host-only engine has no device"; return GM_ERR_NO_DEVICE; }
+    CUDA_TRY(cudaSetDevice(e->device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    CUDA_TRY(cudaMemsetAsync(o->d_needed, 0, 3 * sizeof(uint64_t), s));
+    if (n == 0) return GM_OK;
+    RelParams rp{};
+    rp.spans = reinterpret_cast<const uint2*>(d_spans); rp.ids = d_ids; rp.n = static_cast<u32>(n); rp.pubs = d_publishers;
+    rp.rels = d_rels; rp.n_rels = static_cast<u32>(n_rels);
+    rp.out_spans = reinterpret_cast<uint2*>(o->d_spans); rp.out_rels = o->d_rels; rp.cap_rels = o->cap_rels;
+    rp.out_sub_ids = o->d_sub_ids; rp.cap_sub_ids = o->cap_sub_ids;
+    rp.needed = reinterpret_cast<unsigned long long*>(o->d_needed); rp.status = o->d_status;
+    RelGroups rg{};
+    rg.groups = reinterpret_cast<const uint2*>(gr->d_groups); rg.n_groups = gr->n_groups; rg.members = gr->d_members;
+    rg.online = gr->d_online; rg.n_online_bits = gr->n_online_bits; rg.seed = gr->seed;
+    const unsigned grid = static_cast<unsigned>(std::min<u64>((n + 7) / 8, static_cast<u64>(e->num_sms) * 8));
+    k_relations_choose<<<grid, 256, 0, s>>>(rp, rg);
+    { std::lock_guard<std::mutex> g(e->mu_dev); e->launches++; }
+    CUDA_TRY(cudaGetLastError());
+    return GM_OK;
+}
+
+uint64_t gm_share_key(uint64_t seed, uint32_t row, uint32_t group, uint32_t occ, uint32_t client_key) { return share_key(seed, row, group, occ, client_key); }
 
 int32_t gm_tokenize_batch(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, uint32_t max_tok, uint32_t* out_tokens, uint32_t* out_meta) {
     if (!e || !max_tok || (n && (!offsets || !out_tokens || !out_meta))) return GM_ERR_INVALID_ARG;

@@ -16,7 +16,7 @@ std::string ikey(uint64_t node, const std::string& client, uint64_t tag) { std::
 #define R_TRY0(expr) do { int32_t _rc = (expr); if (_rc != GM_OK) return _rc; } while (0)
 
 GpuRouter::~GpuRouter() {
-    for (Dev* d : {&d_rels_, &d_blob_, &d_offs_, &d_spans_, &d_status_, &d_ids_, &d_needed_, &d_pubs_, &d_ospans_, &d_orels_, &d_subs_})
+    for (Dev* d : {&d_rels_, &d_blob_, &d_offs_, &d_spans_, &d_status_, &d_ids_, &d_needed_, &d_pubs_, &d_ospans_, &d_orels_, &d_subs_, &d_ghdr_, &d_gmem_, &d_online_})
         if (d->p) cudaFree(d->p);
     if (stream_) cudaStreamDestroy(static_cast<cudaStream_t>(stream_));
 }
@@ -31,21 +31,109 @@ int32_t GpuRouter::ensure(Dev& d, size_t bytes) {
     return GM_OK;
 }
 
+// client keys number the (node id, client id) pairs in order of first appearance; a new key starts online
+uint32_t GpuRouter::client_key(uint64_t node_id, const std::string& client) {
+    const uint32_t k = intern(client_key_, ckey(node_id, client));
+    if (online_words_.size() * 32 <= k) {
+        const uint32_t w0 = static_cast<uint32_t>(online_words_.size());
+        online_words_.resize(k / 32 + 1, 0xFFFFFFFFu);
+        online_dirty_.mark(w0, static_cast<uint32_t>(online_words_.size()));
+    }
+    return k;
+}
+
+void GpuRouter::set_online(uint64_t node_id, const std::string& client, bool online) {
+    const uint32_t k = client_key(node_id, client);
+    const uint32_t bit = 1u << (k & 31);
+    online_words_[k / 32] = online ? (online_words_[k / 32] | bit) : (online_words_[k / 32] & ~bit);
+    online_dirty_.mark(k / 32, k / 32 + 1);
+}
+
 // the device record of a relation: everything k_relations needs to apply router.rs:184-200 and types.rs:488-506
 void GpuRouter::set_rel(uint32_t handle, const Rel& r) {
     if (rel_host_.size() <= handle) rel_host_.resize(handle + 1, gm_rel{0, 0, 0, 0, 0});
     gm_rel d{0, 0, 0, 0, 0};
+    uint32_t group = 0;
     if (r.live) {
         d.node_id = r.id.node_id;
-        d.client_key = intern(client_key_, ckey(r.id.node_id, r.client));
+        d.client_key = client_key(r.id.node_id, r.client);
         d.id_idx = intern(id_idx_, ikey(r.id.node_id, r.id.client_id, r.id.tag));
         d.sub_id = r.opts.sub_id;
-        uint32_t group = 0;
-        if (!r.opts.group.empty()) { std::string key = filter_names_[r.filter_idx]; key.push_back('\0'); key += r.opts.group; group = group_index_.emplace(key, static_cast<uint32_t>(group_index_.size() + 1)).first->second; }
+        if (!r.opts.group.empty()) {
+            std::string key = filter_names_[r.filter_idx]; key.push_back('\0'); key += r.opts.group;
+            const auto ins = group_index_.emplace(key, static_cast<uint32_t>(group_index_.size() + 1));
+            group = ins.first->second;
+            if (ins.second) {                                          // a new group: an empty block
+                grp_hdr_.push_back(gm_span{static_cast<uint32_t>(member_pool_.size()), 0}); grp_cap_.push_back(0);
+                grp_filter_.push_back(filter_names_[r.filter_idx]); grp_name_.push_back(r.opts.group);
+                hdr_dirty_.mark(group, group + 1);
+            }
+        }
         d.flags = GM_REL_LIVE | (r.opts.is_v5 ? GM_REL_V5 : 0u) | (r.opts.no_local ? GM_REL_NO_LOCAL : 0u) | (group << 8);
     }
     rel_host_[handle] = d;
     rel_dirty_lo_ = std::min(rel_dirty_lo_, handle); rel_dirty_hi_ = std::max(rel_dirty_hi_, handle + 1);
+    if (member_group_.size() <= handle) { member_group_.resize(handle + 1, 0); member_slot_.resize(handle + 1, 0); }
+    if (member_group_[handle] != group) {                              // a re-subscribe may change or drop the group
+        if (member_group_[handle]) member_remove(handle);
+        if (group) member_add(group, handle);
+    }
+}
+
+void GpuRouter::member_add(uint32_t group, uint32_t handle) {
+    if (grp_hdr_[group].cnt == grp_cap_[group]) {                      // full: the block moves to the pool's end with twice the room
+        const gm_span old = grp_hdr_[group];
+        const uint32_t ncap = std::max<uint32_t>(4, 2 * grp_cap_[group]);
+        const uint32_t noff = static_cast<uint32_t>(member_pool_.size());
+        member_pool_.resize(member_pool_.size() + ncap, 0xFFFFFFFFu);
+        std::copy(member_pool_.begin() + old.off, member_pool_.begin() + old.off + old.cnt, member_pool_.begin() + noff);
+        pool_garbage_ += grp_cap_[group];
+        grp_hdr_[group].off = noff; grp_cap_[group] = ncap;
+        pool_dirty_.mark(noff, noff + old.cnt);
+    }
+    gm_span& b = grp_hdr_[group];
+    member_pool_[b.off + b.cnt] = handle;
+    member_group_[handle] = group; member_slot_[handle] = b.cnt;
+    pool_dirty_.mark(b.off + b.cnt, b.off + b.cnt + 1);
+    b.cnt++;
+    hdr_dirty_.mark(group, group + 1);
+    groups_changed_ = true;
+    if (pool_garbage_ > 4096 && pool_garbage_ * 2 > member_pool_.size()) repack_groups();
+}
+
+void GpuRouter::member_remove(uint32_t handle) {                       // the block's last entry takes the freed slot
+    const uint32_t group = member_group_[handle];
+    gm_span& b = grp_hdr_[group];
+    const uint32_t slot = member_slot_[handle], last = member_pool_[b.off + b.cnt - 1];
+    member_pool_[b.off + slot] = last; member_slot_[last] = slot;
+    member_pool_[b.off + b.cnt - 1] = 0xFFFFFFFFu;
+    b.cnt--;
+    member_group_[handle] = 0;
+    pool_dirty_.mark(b.off + slot, b.off + slot + 1);
+    hdr_dirty_.mark(group, group + 1);
+    groups_changed_ = true;
+}
+
+void GpuRouter::repack_groups() {
+    std::vector<uint32_t> pool;
+    for (size_t g = 1; g < grp_hdr_.size(); ++g) {
+        const gm_span old = grp_hdr_[g];
+        const uint32_t off = static_cast<uint32_t>(pool.size());
+        pool.insert(pool.end(), member_pool_.begin() + old.off, member_pool_.begin() + old.off + old.cnt);
+        pool.resize(off + grp_cap_[g], 0xFFFFFFFFu);
+        grp_hdr_[g].off = off;
+    }
+    member_pool_.swap(pool);
+    pool_garbage_ = 0;
+    hdr_dirty_.mark(0, static_cast<uint32_t>(grp_hdr_.size()));
+    pool_dirty_.mark(0, static_cast<uint32_t>(member_pool_.size()));
+}
+
+bool GpuRouter::group(uint32_t g, const std::string** filter, const std::string** name, const uint32_t** members, uint32_t* cnt) const {
+    if (g == 0 || g >= grp_hdr_.size()) return false;
+    *filter = &grp_filter_[g]; *name = &grp_name_[g];
+    *members = member_pool_.data() + grp_hdr_[g].off; *cnt = grp_hdr_[g].cnt;
+    return true;
 }
 
 int32_t GpuRouter::add(const char* filter, uint32_t len, const Id& id, const Opts& opts) {
@@ -184,15 +272,55 @@ int32_t GpuRouter::host_dedup_topic(const gm_sub_relation* in, uint32_t cnt, std
     return GM_OK;
 }
 
+// the same for a topic of the choosing form: chosen v5 members (group field set) are de-duplicated like any other v5 relation, and
+// the client's smallest handle represents it, as on the device
+int32_t GpuRouter::host_dedup_topic_chosen(const gm_sub_relation* in, uint32_t cnt, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids) {
+    struct V5Entry { size_t rel_pos; std::vector<uint32_t> ids; };
+    std::unordered_map<uint32_t, V5Entry> v5;
+    for (uint32_t k = 0; k < cnt; ++k) {
+        const uint32_t h = in[k].handle;
+        const gm_rel& d = rel_host_[h];
+        if (!(d.flags & GM_REL_V5)) { rels.push_back(gm_sub_relation{d.node_id, h, in[k].group, 0, 0}); continue; }
+        auto it = v5.find(d.client_key);
+        if (it == v5.end()) it = v5.emplace(d.client_key, V5Entry{rels.size(), {}}).first, rels.push_back(gm_sub_relation{d.node_id, h, in[k].group, 0, 0});
+        else if (h < rels[it->second.rel_pos].handle) rels[it->second.rel_pos] = gm_sub_relation{d.node_id, h, in[k].group, 0, 0};
+        if (d.sub_id) it->second.ids.push_back(d.sub_id);
+    }
+    for (auto& kv : v5) {
+        gm_sub_relation& sr = rels[kv.second.rel_pos];
+        sr.sub_ids_off = static_cast<uint32_t>(sub_ids.size()); sr.sub_ids_cnt = static_cast<uint32_t>(kv.second.ids.size());
+        sub_ids.insert(sub_ids.end(), kv.second.ids.begin(), kv.second.ids.end());
+    }
+    return GM_OK;
+}
+
 #define R_CUDA(expr) do { cudaError_t _ce = (expr); if (_ce != cudaSuccess) return (_ce == cudaErrorNoDevice || _ce == cudaErrorInsufficientDriver) ? GM_ERR_NO_DEVICE : GM_ERR_CUDA; } while (0)
 #define R_TRY(expr) do { int32_t _rc = (expr); if (_rc != GM_OK) return _rc; } while (0)
+
+// the group header, member pool and online bitmap: what changed since the last choosing call
+int32_t GpuRouter::ship_groups(void* stream) {
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    auto ship = [&](Dev& d, const void* host, size_t elem, size_t count, Dirty& dirty) -> int32_t {
+        R_TRY(ensure(d, std::max<size_t>(count, 256) * elem));
+        if (dirty.any()) {
+            const size_t lo = dirty.lo, hi = std::min<size_t>(dirty.hi, count);
+            if (hi > lo) R_CUDA(cudaMemcpyAsync(static_cast<char*>(d.p) + lo * elem, static_cast<const char*>(host) + lo * elem, (hi - lo) * elem, cudaMemcpyHostToDevice, s));
+            dirty = Dirty{};
+        }
+        return GM_OK;
+    };
+    R_TRY(ship(d_ghdr_, grp_hdr_.data(), sizeof(gm_span), grp_hdr_.size(), hdr_dirty_));
+    R_TRY(ship(d_gmem_, member_pool_.data(), 4, member_pool_.size(), pool_dirty_));
+    R_TRY(ship(d_online_, online_words_.data(), 4, online_words_.size(), online_dirty_));
+    return GM_OK;
+}
 
 // Router::matches for a batch.  Everything per relation happens on the device (engine match, then k_relations writes the
 // finished gm_sub_relation records); the records are copied straight into the caller's arrays.  Returns GM_ERR_CAPACITY with
 // *needed_* set when an output is too small.
 int32_t GpuRouter::matches_batch(const gm_id* publishers, const char* blob, const uint32_t* offs, uint64_t n, gm_span* out_spans,
                                  gm_sub_relation* out_rels, uint64_t cap_rels, uint32_t* out_sub_ids, uint64_t cap_sub_ids,
-                                 uint64_t* needed_rels, uint64_t* needed_sub_ids, int32_t* status) {
+                                 uint64_t* needed_rels, uint64_t* needed_sub_ids, int32_t* status, const uint64_t* share_seed) {
     if (needed_rels) *needed_rels = 0;
     if (needed_sub_ids) *needed_sub_ids = 0;
     if (n == 0) return GM_OK;
@@ -200,6 +328,11 @@ int32_t GpuRouter::matches_batch(const gm_id* publishers, const char* blob, cons
     const auto t0 = Clk::now();
     if (!stream_) { cudaStream_t s; R_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); stream_ = s; }
     cudaStream_t s = static_cast<cudaStream_t>(stream_);
+    if (share_seed) {
+        // a group's representative must be in the device trie, also on an engine that only flushes when told to
+        if (groups_changed_) { R_TRY(gm_flush(e_)); groups_changed_ = false; unflushed_removes_ = false; }
+        R_TRY(ship_groups(s));
+    }
     // ---- the relation table: ship what changed since the last call
     if (rel_dirty_hi_ > rel_dirty_lo_) {
         R_TRY(ensure(d_rels_, std::max<size_t>(rel_host_.size(), 1024) * sizeof(gm_rel)));
@@ -242,8 +375,15 @@ int32_t GpuRouter::matches_batch(const gm_id* publishers, const char* blob, cons
     o.d_spans = static_cast<gm_span*>(d_ospans_.p); o.d_rels = static_cast<gm_sub_relation*>(d_orels_.p); o.cap_rels = d_orels_.cap / sizeof(gm_sub_relation);
     o.d_sub_ids = static_cast<uint32_t*>(d_subs_.p); o.cap_sub_ids = d_subs_.cap / 4;
     o.d_needed = static_cast<uint64_t*>(d_needed_.p); o.d_status = static_cast<int32_t*>(d_status_.p);
-    R_TRY(gm_relations_expand_device(e_, static_cast<const gm_span*>(d_spans_.p), static_cast<const uint32_t*>(d_ids_.p), n, publishers ? static_cast<const uint32_t*>(d_pubs_.p) : nullptr,
-                                     static_cast<const gm_rel*>(d_rels_.p), rel_host_.size(), &o, s));
+    if (share_seed) {
+        gm_rel_groups gr{};
+        gr.d_groups = static_cast<const gm_span*>(d_ghdr_.p); gr.n_groups = static_cast<uint32_t>(grp_hdr_.size()); gr.d_members = static_cast<const uint32_t*>(d_gmem_.p);
+        gr.d_online = static_cast<const uint32_t*>(d_online_.p); gr.n_online_bits = static_cast<uint32_t>(client_key_.size()); gr.seed = *share_seed;
+        R_TRY(gm_relations_choose_device(e_, static_cast<const gm_span*>(d_spans_.p), static_cast<const uint32_t*>(d_ids_.p), n, publishers ? static_cast<const uint32_t*>(d_pubs_.p) : nullptr,
+                                         static_cast<const gm_rel*>(d_rels_.p), rel_host_.size(), &gr, &o, s));
+    } else
+        R_TRY(gm_relations_expand_device(e_, static_cast<const gm_span*>(d_spans_.p), static_cast<const uint32_t*>(d_ids_.p), n, publishers ? static_cast<const uint32_t*>(d_pubs_.p) : nullptr,
+                                         static_cast<const gm_rel*>(d_rels_.p), rel_host_.size(), &o, s));
     R_CUDA(cudaMemcpyAsync(need, d_needed_.p, 2 * 8, cudaMemcpyDeviceToHost, s));
     R_CUDA(cudaMemcpyAsync(status, d_status_.p, n * 4, cudaMemcpyDeviceToHost, s));
     R_CUDA(cudaMemcpyAsync(out_spans, d_ospans_.p, n * 8, cudaMemcpyDeviceToHost, s));
@@ -272,7 +412,7 @@ int32_t GpuRouter::matches_batch(const gm_id* publishers, const char* blob, cons
     for (uint64_t i = 0; i < n; ++i) {
         const size_t begin = rels.size();
         const uint32_t off = out_spans[i].off, cnt = out_spans[i].cnt;
-        if (status[i] == 1) { status[i] = 0; R_TRY(host_dedup_topic(dev.data() + off, cnt, rels, sub_ids)); }
+        if (status[i] == 1) { status[i] = 0; R_TRY(share_seed ? host_dedup_topic_chosen(dev.data() + off, cnt, rels, sub_ids) : host_dedup_topic(dev.data() + off, cnt, rels, sub_ids)); }
         else if (status[i] == 0)
             for (uint32_t k = 0; k < cnt; ++k) {
                 gm_sub_relation sr = dev[off + k];

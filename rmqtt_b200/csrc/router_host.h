@@ -11,9 +11,11 @@
 //             k_relations (relations.cuh): no_local (:184-189), shared-group members passed through (:192-200),
 //             v5 per-client de-dup with accumulation of subscription identifiers (types.rs:488-506) -> the host only
 //             receives the finished gm_sub_relation records by DMA.  The router keeps a 24-byte gm_rel record per
-//             handle in HBM (shipped incrementally).  The shared-subscription *choice* is rand::random in the
-//             reference (subscribe.rs:88): members are returned, not chosen.
+//             handle in HBM (shipped incrementally).  matches_batch returns every shared-group member; with a seed
+//             it chooses one per group on the device (k_relations_choose, subscribe.rs:66-104 with a seeded draw),
+//             from per-group member blocks and an online bitmap the router keeps in device layout.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <mutex>
 #include <string>
@@ -39,9 +41,12 @@ class GpuRouter {
     int32_t remove(const char* filter, uint32_t len, const Id& id, bool* removed);
     int64_t topics() const { return topics_; }                // Router::topics  (router.rs:554-556)
     int64_t routes() const { return routes_; }                // Router::routes
+    // share_seed: null returns every shared-group member; else one member per group is chosen with that seed
     int32_t matches_batch(const gm_id* publishers, const char* blob, const uint32_t* offs, uint64_t n, gm_span* out_spans,
                           gm_sub_relation* out_rels, uint64_t cap_rels, uint32_t* out_sub_ids, uint64_t cap_sub_ids,
-                          uint64_t* needed_rels, uint64_t* needed_sub_ids, int32_t* status);
+                          uint64_t* needed_rels, uint64_t* needed_sub_ids, int32_t* status, const uint64_t* share_seed = nullptr);
+    void set_online(uint64_t node_id, const std::string& client, bool online);        // Router::is_online
+    bool group(uint32_t group, const std::string** filter, const std::string** name, const uint32_t** members, uint32_t* cnt) const;
     bool relation(uint32_t handle, const std::string** filter, const std::string** client) const;
     // unique matched filters per topic, through the engine's descriptor mode (router.rs:139-158, 315-363, 522-546)
     int32_t matched_filters_batch(const char* blob, const uint32_t* offs, uint64_t n, std::vector<gm_span>& spans, std::vector<uint32_t>& filters,
@@ -70,10 +75,30 @@ class GpuRouter {
     Dev d_rels_, d_blob_, d_offs_, d_spans_, d_status_, d_ids_, d_needed_, d_pubs_, d_ospans_, d_orels_, d_subs_;
     std::vector<uint32_t> pubs_;
     void* stream_ = nullptr;
+    // ---- shared groups in device layout (k_relations_choose): group id -> a block of live member handles with spare room in one
+    //      pool; a block that fills up moves to the pool's end, and the pool is re-packed once the abandoned blocks pass half of it.
+    //      The header, the pool and the online bitmap are shipped by dirty range, like rel_host_.
+    struct Dirty { uint32_t lo = 0xFFFFFFFFu, hi = 0; void mark(uint32_t a, uint32_t b) { lo = std::min(lo, a); hi = std::max(hi, b); } bool any() const { return hi > lo; } };
+    std::vector<gm_span> grp_hdr_{gm_span{0, 0}};                      // group id -> {off, cnt} in member_pool_; [0] unused
+    std::vector<uint32_t> grp_cap_{0};                                 // group id -> block capacity
+    std::vector<std::string> grp_filter_{std::string()}, grp_name_{std::string()};
+    std::vector<uint32_t> member_pool_;
+    std::vector<uint32_t> member_group_, member_slot_;                 // handle -> group it is listed in (0: none), its index in the block
+    uint64_t pool_garbage_ = 0;
+    Dirty hdr_dirty_, pool_dirty_, online_dirty_;                      // online_dirty_ counts words
+    bool groups_changed_ = false;                                      // membership changed since the router's last gm_flush
+    std::vector<uint32_t> online_words_;                               // bit per client_key, 1 = online
+    Dev d_ghdr_, d_gmem_, d_online_;
     int32_t ensure(Dev& d, size_t bytes);
     uint32_t intern(std::unordered_map<std::string, uint32_t>& m, const std::string& k) { return m.emplace(k, static_cast<uint32_t>(m.size())).first->second; }
+    uint32_t client_key(uint64_t node_id, const std::string& client);
     void set_rel(uint32_t handle, const Rel& r);
+    void member_add(uint32_t group, uint32_t handle);
+    void member_remove(uint32_t handle);
+    void repack_groups();
+    int32_t ship_groups(void* stream);
     int32_t host_dedup_topic(const gm_sub_relation* in, uint32_t cnt, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids);
+    int32_t host_dedup_topic_chosen(const gm_sub_relation* in, uint32_t cnt, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids);
 };
 
 }  // namespace gm

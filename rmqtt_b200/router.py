@@ -36,7 +36,9 @@ class SubRelation:
     topic_filter: str
     client_id: str
     sub_ids: list = field(default_factory=list)
-    group: int = 0          # 0, or id of the (filter, shared group) whose member this is: the caller chooses one per group
+    group: int = 0          # 0, or id of the (filter, shared group) whose member this is: matches_batch returns every member,
+                            # matches_batch_shared the chosen one
+    online: bool = True     # matches_batch_shared: False when no eligible member of the group was online
 
 
 class GpuRouter:
@@ -91,8 +93,28 @@ class GpuRouter:
         self._check(self._lib.gmr_relation(self._h, handle, C.byref(f), C.byref(fl), C.byref(c), C.byref(cl)))
         return C.string_at(f, fl.value).decode(), C.string_at(c, cl.value).decode()
 
-    def matches_batch(self, topics, publishers=None):
-        """Router::matches for a batch -> list (per topic) of list[SubRelation], or None for an invalid topic."""
+    def set_online(self, node_id: int, client_id: str, online: bool):
+        """What Router::is_online answers for (node_id, client_id); a client never named here is online."""
+        c = _b(client_id)
+        self._check(self._lib.gmr_set_online(self._h, node_id, c, len(c), int(bool(online))))
+
+    def group_members(self, group: int):
+        """-> (filter, group name, member handles) of a shared group id (the group_cids of SharedGroupType)."""
+        f, g = C.c_char_p(), C.c_char_p()
+        fl, gl, n = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+        self._check(self._lib.gmr_group(self._h, group, C.byref(f), C.byref(fl), C.byref(g), C.byref(gl), None, 0, C.byref(n)))
+        hs = np.zeros(max(1, n.value), dtype=np.uint32)
+        self._check(self._lib.gmr_group(self._h, group, C.byref(f), C.byref(fl), C.byref(g), C.byref(gl), hs.ctypes.data_as(C.c_void_p), n.value, C.byref(n)))
+        return C.string_at(f, fl.value).decode(), C.string_at(g, gl.value).decode(), [int(x) for x in hs[:n.value]]
+
+    def matches_batch_shared(self, topics, publishers=None, seed: int = 0):
+        """Router::matches for a batch with ONE member chosen per matched (filter, shared group), on the device: the draw of
+        include/gpumqtt.h gm_relations_choose_device, reproducible from `seed`."""
+        return self.matches_batch(topics, publishers, seed=seed)
+
+    def matches_batch(self, topics, publishers=None, *, seed: int | None = None):
+        """Router::matches for a batch -> list (per topic) of list[SubRelation], or None for an invalid topic.  Every shared-group
+        member is returned unless `seed` is given (see matches_batch_shared)."""
         blob, offs = pack(topics)
         n = len(topics)
         pubs = None
@@ -111,9 +133,12 @@ class GpuRouter:
             rels = (N.GmSubRelation * cap_r)()
             sids = np.zeros(cap_s, dtype=np.uint32)
             nr, ns = C.c_uint64(0), C.c_uint64(0)
-            rc = self._lib.gmr_matches_batch(self._h, pubs, blob.ctypes.data_as(C.c_void_p), offs.ctypes.data_as(C.c_void_p), n,
-                                             spans.ctypes.data_as(C.c_void_p), rels, cap_r, sids.ctypes.data_as(C.c_void_p), cap_s,
-                                             C.byref(nr), C.byref(ns), status.ctypes.data_as(C.c_void_p))
+            args = (pubs, blob.ctypes.data_as(C.c_void_p), offs.ctypes.data_as(C.c_void_p), n, spans.ctypes.data_as(C.c_void_p), rels, cap_r,
+                    sids.ctypes.data_as(C.c_void_p), cap_s, C.byref(nr), C.byref(ns), status.ctypes.data_as(C.c_void_p))
+            if seed is None:
+                rc = self._lib.gmr_matches_batch(self._h, *args)
+            else:
+                rc = self._lib.gmr_matches_batch_shared(self._h, seed, *args)
             if rc == N.GM_ERR_CAPACITY:
                 cap_r, cap_s = int(nr.value) + 16, int(ns.value) + 16
                 continue
@@ -128,7 +153,8 @@ class GpuRouter:
             for k in range(int(spans[i, 0]), int(spans[i, 0] + spans[i, 1])):
                 r = rels[k]
                 f, c = self._relation(r.handle)
-                lst.append(SubRelation(int(r.node_id), f, c, sids[r.sub_ids_off:r.sub_ids_off + r.sub_ids_cnt].tolist(), int(r.group)))
+                lst.append(SubRelation(int(r.node_id), f, c, sids[r.sub_ids_off:r.sub_ids_off + r.sub_ids_cnt].tolist(),
+                                       int(r.group) & ~N.GM_SUBREL_OFFLINE, not (int(r.group) & N.GM_SUBREL_OFFLINE)))
             out.append(lst)
         return out
 
