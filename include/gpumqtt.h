@@ -241,6 +241,8 @@ int32_t gmr_last_timing(gm_router* r, double* device_ms, double* host_ms);
 int64_t gmr_topics(gm_router* r);
 int64_t gmr_routes(gm_router* r);
 /* Router::matches for a batch; publishers[i] is the `this_id` of PUBLISH i (NULL: no no_local filtering).
+ * A v5 client that matches through several subscriptions gets one record, carrying the client's smallest matched handle and
+ * the subscription ids of all of them; gmr_matches_batch_shared merges the same way.
  * Returns GM_ERR_CAPACITY with *needed_rels / *needed_sub_ids set when an output is too small.               */
 int32_t gmr_matches_batch(gm_router* r, const gm_id* publishers, const char* topics_blob, const uint32_t* topic_offsets, uint64_t n,
                           gm_span* out_spans, gm_sub_relation* out_rels, uint64_t cap_rels, uint32_t* out_sub_ids, uint64_t cap_sub_ids,
@@ -353,7 +355,8 @@ typedef struct gm_rel {           /* one subscription relation, indexed by its h
 #define GM_REL_NO_LOCAL 4u
 typedef struct gm_rel_out {
     gm_span* d_spans;             /* [n] per topic: its relations in d_rels */
-    gm_sub_relation* d_rels; uint64_t cap_rels;      /* finished records: node id, handle, group, sub-id range */
+    gm_sub_relation* d_rels; uint64_t cap_rels;      /* finished records: node id, handle, group, sub-id range; a record merged
+                                                        per client carries the client's smallest handle (both calls) */
     uint32_t* d_sub_ids; uint64_t cap_sub_ids;
     uint64_t* d_needed;           /* device [3]: relations, sub ids produced, (unused) — capacity protocol: compare on the host, retry */
     int32_t* d_status;            /* [n]: set to 1 where a topic had more v5 relations than the kernel stages (256): that topic's list is

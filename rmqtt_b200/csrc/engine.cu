@@ -1484,31 +1484,10 @@ int32_t gm_device_read(gm_engine* e, const void* d_src, void* h_dst, uint64_t by
     return GM_OK;
 }
 
-int32_t gm_relations_expand_device(gm_engine* e, const gm_span* d_spans, const uint32_t* d_ids, uint64_t n, const uint32_t* d_publishers,
-                                   const gm_rel* d_rels, uint64_t n_rels, const gm_rel_out* o, void* stream) {
-    if (!e || !o || !o->d_needed || (n && (!d_spans || !o->d_spans || !o->d_status))) return GM_ERR_INVALID_ARG;
-    if (n > 0xFFFFFFF0ull || n_rels > 0xFFFFFFFFull) { g_err = "batch too large"; return GM_ERR_TOO_LARGE; }
-    if (e->flags & GM_FLAG_HOST_ONLY) { g_err = "host-only engine has no device"; return GM_ERR_NO_DEVICE; }
-    CUDA_TRY(cudaSetDevice(e->device));
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(cudaMemsetAsync(o->d_needed, 0, 3 * sizeof(uint64_t), s));
-    if (n == 0) return GM_OK;
-    RelParams rp{};
-    rp.spans = reinterpret_cast<const uint2*>(d_spans); rp.ids = d_ids; rp.n = static_cast<u32>(n); rp.pubs = d_publishers;
-    rp.rels = d_rels; rp.n_rels = static_cast<u32>(n_rels);
-    rp.out_spans = reinterpret_cast<uint2*>(o->d_spans); rp.out_rels = o->d_rels; rp.cap_rels = o->cap_rels;
-    rp.out_sub_ids = o->d_sub_ids; rp.cap_sub_ids = o->cap_sub_ids;
-    rp.needed = reinterpret_cast<unsigned long long*>(o->d_needed); rp.status = o->d_status;
-    const unsigned grid = static_cast<unsigned>(std::min<u64>((n + 7) / 8, static_cast<u64>(e->num_sms) * 8));
-    k_relations<<<grid, 256, 0, s>>>(rp);
-    { std::lock_guard<std::mutex> g(e->mu_dev); e->launches++; }
-    CUDA_TRY(cudaGetLastError());
-    return GM_OK;
-}
-
-int32_t gm_relations_choose_device(gm_engine* e, const gm_span* d_spans, const uint32_t* d_ids, uint64_t n, const uint32_t* d_publishers,
-                                   const gm_rel* d_rels, uint64_t n_rels, const gm_rel_groups* gr, const gm_rel_out* o, void* stream) {
-    if (!e || !o || !gr || !o->d_needed || (n && (!d_spans || !o->d_spans || !o->d_status)) || (gr->n_groups && (!gr->d_groups || !gr->d_members)))
+// gm_relations_expand_device (gr = null) and gm_relations_choose_device
+static int32_t relations_device(gm_engine* e, const gm_span* d_spans, const uint32_t* d_ids, uint64_t n, const uint32_t* d_publishers,
+                                const gm_rel* d_rels, uint64_t n_rels, const gm_rel_groups* gr, const gm_rel_out* o, void* stream) {
+    if (!e || !o || !o->d_needed || (n && (!d_spans || !o->d_spans || !o->d_status)) || (gr && gr->n_groups && (!gr->d_groups || !gr->d_members)))
         return GM_ERR_INVALID_ARG;
     if (n > 0xFFFFFFF0ull || n_rels > 0xFFFFFFFFull) { g_err = "batch too large"; return GM_ERR_TOO_LARGE; }
     if (e->flags & GM_FLAG_HOST_ONLY) { g_err = "host-only engine has no device"; return GM_ERR_NO_DEVICE; }
@@ -1516,20 +1495,21 @@ int32_t gm_relations_choose_device(gm_engine* e, const gm_span* d_spans, const u
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaMemsetAsync(o->d_needed, 0, 3 * sizeof(uint64_t), s));
     if (n == 0) return GM_OK;
-    RelParams rp{};
-    rp.spans = reinterpret_cast<const uint2*>(d_spans); rp.ids = d_ids; rp.n = static_cast<u32>(n); rp.pubs = d_publishers;
-    rp.rels = d_rels; rp.n_rels = static_cast<u32>(n_rels);
-    rp.out_spans = reinterpret_cast<uint2*>(o->d_spans); rp.out_rels = o->d_rels; rp.cap_rels = o->cap_rels;
-    rp.out_sub_ids = o->d_sub_ids; rp.cap_sub_ids = o->cap_sub_ids;
-    rp.needed = reinterpret_cast<unsigned long long*>(o->d_needed); rp.status = o->d_status;
-    RelGroups rg{};
-    rg.groups = reinterpret_cast<const uint2*>(gr->d_groups); rg.n_groups = gr->n_groups; rg.members = gr->d_members;
-    rg.online = gr->d_online; rg.n_online_bits = gr->n_online_bits; rg.seed = gr->seed;
-    const unsigned grid = static_cast<unsigned>(std::min<u64>((n + 7) / 8, static_cast<u64>(e->num_sms) * 8));
-    k_relations_choose<<<grid, 256, 0, s>>>(rp, rg);
+    launch_relations(d_spans, d_ids, n, d_publishers, d_rels, n_rels, gr, *o, e->num_sms, s);
     { std::lock_guard<std::mutex> g(e->mu_dev); e->launches++; }
     CUDA_TRY(cudaGetLastError());
     return GM_OK;
+}
+
+int32_t gm_relations_expand_device(gm_engine* e, const gm_span* d_spans, const uint32_t* d_ids, uint64_t n, const uint32_t* d_publishers,
+                                   const gm_rel* d_rels, uint64_t n_rels, const gm_rel_out* o, void* stream) {
+    return relations_device(e, d_spans, d_ids, n, d_publishers, d_rels, n_rels, nullptr, o, stream);
+}
+
+int32_t gm_relations_choose_device(gm_engine* e, const gm_span* d_spans, const uint32_t* d_ids, uint64_t n, const uint32_t* d_publishers,
+                                   const gm_rel* d_rels, uint64_t n_rels, const gm_rel_groups* gr, const gm_rel_out* o, void* stream) {
+    if (!gr) return GM_ERR_INVALID_ARG;
+    return relations_device(e, d_spans, d_ids, n, d_publishers, d_rels, n_rels, gr, o, stream);
 }
 
 uint64_t gm_share_key(uint64_t seed, uint32_t row, uint32_t group, uint32_t occ, uint32_t client_key) { return share_key(seed, row, group, occ, client_key); }

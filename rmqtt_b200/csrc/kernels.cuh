@@ -17,6 +17,13 @@
 
 #include "layout.h"
 
+// a kernel launch; the CPU emulation (tests/native/emu, -DGM_CPU_EMU) runs the same kernel over host memory
+#ifdef GM_CPU_EMU
+#define GM_LAUNCH(k, grid, block, smem, s, ...) emu::launch(dim3(grid), dim3(block), [&] { k(__VA_ARGS__); })
+#else
+#define GM_LAUNCH(k, grid, block, smem, s, ...) k<<<grid, block, smem, s>>>(__VA_ARGS__)
+#endif
+
 namespace gm {
 
 struct MatchParams {

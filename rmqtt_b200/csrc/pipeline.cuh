@@ -12,12 +12,6 @@
 #include "retain_kernels.cuh"
 #include "retain_tree.h"
 
-#ifdef GM_CPU_EMU
-#define GM_LAUNCH(k, grid, block, smem, s, ...) emu::launch(dim3(grid), dim3(block), [&] { k(__VA_ARGS__); })
-#else
-#define GM_LAUNCH(k, grid, block, smem, s, ...) k<<<grid, block, smem, s>>>(__VA_ARGS__)
-#endif
-
 namespace gm {
 
 // ---- control blocks ----------------------------------------------------------------------------------------------------

@@ -3,8 +3,8 @@
 //
 //   * `no_local` (router.rs:184-189): a v5 subscriber that set no_local does not receive its own PUBLISH — the relation is
 //     dropped when the publisher's Id equals the subscriber's Id;
-//   * shared-subscription members (router.rs:192-200) and v3 relations pass through in k_relations; k_relations_choose
-//     (below) also makes the choice of ONE member per group (router.rs:224-238) with a seeded draw;
+//   * shared-subscription members (router.rs:192-200) and v3 relations pass through in k_relations<false>; k_relations<true>
+//     instead makes the choice of ONE member per group (router.rs:224-238) with a seeded draw;
 //   * v5 relations are de-duplicated PER CLIENT (types.rs:488-506): a client that matches through several filters gets ONE
 //     relation, and the subscription identifiers of all its matching subscriptions accumulate.
 //
@@ -15,6 +15,8 @@
 // than REL_STAGE v5 relations is flagged (status 1) and handed to the host un-deduplicated.
 #pragma once
 #include <cuda_runtime.h>
+
+#include <algorithm>
 
 #include "../../include/gpumqtt.h"
 #include "kernels.cuh"
@@ -46,100 +48,6 @@ __device__ __forceinline__ gm_rel load_rel(const gm_rel* p) {      // 24-byte re
     gm_rel r;
     r.node_id = (static_cast<unsigned long long>(a.y) << 32) | a.x; r.client_key = b.x; r.id_idx = b.y; r.sub_id = c.x; r.flags = c.y;
     return r;
-}
-
-__global__ void __launch_bounds__(256)
-k_relations(RelParams p) {
-    __shared__ u32 s_key[8][REL_STAGE], s_h[8][REL_STAGE], s_sub[8][REL_STAGE];
-    const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5, lt = lanemask_lt();
-    const u32 gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-    u32* sk = s_key[wid]; u32* sh = s_h[wid]; u32* ss = s_sub[wid];
-    for (u32 t = gwarp; t < p.n; t += nwarps) {
-        const uint2 sp = p.spans[t];
-        const u32 off = sp.x, cnt = sp.y;
-        const u32 pub = p.pubs ? p.pubs[t] : REL_NONE;
-        // classify one handle: 0 dropped, 1 direct (v3 / shared-group member), 2 v5 relation subject to per-client de-dup
-        auto classify = [&](u32 i, u32& h, gm_rel& r) -> u32 {
-            if (i >= cnt) return 0u;
-            h = p.ids[off + i];
-            if (h >= p.n_rels) return 0u;
-            r = load_rel(p.rels + h);
-            if (!(r.flags & GM_REL_LIVE)) return 0u;
-            if ((r.flags & GM_REL_V5) && (r.flags & GM_REL_NO_LOCAL) && pub != REL_NONE && r.id_idx == pub) return 0u;   // router.rs:184-189
-            return ((r.flags & GM_REL_V5) && (r.flags >> 8) == 0u) ? 2u : 1u;
-        };
-        // ---- pass 1: count, stage the v5 relations ----
-        u32 ndirect = 0, nv = 0;
-        for (u32 i0 = 0; i0 < cnt; i0 += 32) {
-            u32 h = 0; gm_rel r{};
-            const u32 c = classify(i0 + lane, h, r);
-            ndirect += __popc(__ballot_sync(0xFFFFFFFFu, c == 1u));
-            const u32 bv = __ballot_sync(0xFFFFFFFFu, c == 2u);
-            if (c == 2u) { const u32 at = nv + __popc(bv & lt); if (at < REL_STAGE) { sk[at] = r.client_key; sh[at] = h; ss[at] = r.sub_id; } }
-            nv += __popc(bv);
-        }
-        __syncwarp();
-        const bool overflow = nv > REL_STAGE;
-        // ---- de-dup: entry e represents its client iff it holds the smallest handle of the client's relations (the same handle can
-        //      occur twice: a topic with a literal '+' / '#' level visits a wildcard child twice — ties go to the earlier entry) ----
-        u32 nreps = 0, nsubs = 0;
-        if (!overflow) {
-            for (u32 e0 = 0; e0 < nv; e0 += 32) {
-                const u32 e = e0 + lane;
-                bool rep = false; u32 nsub = 0;
-                if (e < nv) {
-                    const u32 key = sk[e], h = sh[e];
-                    rep = true;
-                    for (u32 j = 0; j < nv; ++j) if (sk[j] == key) { rep &= !(sh[j] < h || (sh[j] == h && j < e)); nsub += ss[j] != 0u; }
-                }
-                nreps += __popc(__ballot_sync(0xFFFFFFFFu, rep));
-                nsubs += __reduce_add_sync(0xFFFFFFFFu, rep ? nsub : 0u);
-            }
-        } else nreps = nv;                       // handed over un-deduplicated
-        const u32 total = ndirect + nreps;
-        unsigned long long hb = 0, sb = 0;
-        if (lane == 0) {
-            if (total) hb = atomicAdd(p.needed + 0, static_cast<unsigned long long>(total));
-            if (nsubs) sb = atomicAdd(p.needed + 1, static_cast<unsigned long long>(nsubs));
-        }
-        hb = __shfl_sync(0xFFFFFFFFu, hb, 0); sb = __shfl_sync(0xFFFFFFFFu, sb, 0);
-        const bool fits = hb + total <= p.cap_rels && sb + nsubs <= p.cap_sub_ids && hb + total <= 0xFFFFFFFFull && sb + nsubs <= 0xFFFFFFFFull;
-        if (lane == 0) { p.out_spans[t] = make_uint2(fits ? static_cast<u32>(hb) : 0u, total); if (overflow) p.status[t] = 1; }
-        if (!fits || total == 0) { __syncwarp(); continue; }
-        // ---- pass 2: write the finished gm_sub_relation records.  Direct relations first (after an overflow, the v5 ones with them) ----
-        u32 w = 0;
-        for (u32 i0 = 0; i0 < cnt; i0 += 32) {
-            u32 h = 0; gm_rel r{};
-            const u32 c = classify(i0 + lane, h, r);
-            const bool take = c == 1u || (overflow && c == 2u);
-            const u32 b = __ballot_sync(0xFFFFFFFFu, take);
-            if (take) p.out_rels[hb + w + __popc(b & lt)] = gm_sub_relation{r.node_id, h, r.flags >> 8, 0u, 0u};
-            w += __popc(b);
-        }
-        if (!overflow) {
-            u32 ws = 0;
-            for (u32 e0 = 0; e0 < nv; e0 += 32) {
-                const u32 e = e0 + lane;
-                bool rep = false; u32 nsub = 0, key = 0, h = 0;
-                if (e < nv) {
-                    key = sk[e]; h = sh[e];
-                    rep = true;
-                    for (u32 j = 0; j < nv; ++j) if (sk[j] == key) { rep &= !(sh[j] < h || (sh[j] == h && j < e)); nsub += ss[j] != 0u; }
-                }
-                const u32 br = __ballot_sync(0xFFFFFFFFu, rep);
-                const u32 mys = rep ? nsub : 0u;
-                const u32 inc = warp_incl_scan(mys, lane);
-                if (rep) {
-                    const u32 so = static_cast<u32>(sb) + ws + (inc - mys);
-                    p.out_rels[hb + w + __popc(br & lt)] = gm_sub_relation{load_rel(p.rels + h).node_id, h, 0u, nsub ? so : 0u, nsub};
-                    u32 k = 0;
-                    for (u32 j = 0; j < nv && k < nsub; ++j) if (sk[j] == key && ss[j] != 0u) p.out_sub_ids[so + k++] = ss[j];   // types.rs:497-503
-                }
-                w += __popc(br); ws += __shfl_sync(0xFFFFFFFFu, inc, 31);
-            }
-        }
-        __syncwarp();
-    }
 }
 
 // ---- shared subscriptions: ONE member per (matched filter, group) and appearance (router.rs:192-238, subscribe.rs:66-104) ----
@@ -201,15 +109,19 @@ __device__ __forceinline__ u32 share_choose(const RelParams& p, const RelGroups&
     return best.h;
 }
 
-// k_relations with the choice made on the device.  In a row's match list a shared member stands for its group only if it is
-// the group's REPRESENTATIVE (members[groups[g].off]); every other member entry is dropped.  Every matched filter node emits
-// its whole value set, so the representative appears once per appearance of the group.  Per appearance the warp scans the
-// group's block and chooses; a chosen v3 member is a direct record, a chosen v5 member joins the row's v5 relations and is
-// de-duplicated per client with them (types.rs:488-506).  A chosen record's group field is the group id | GM_SUBREL_OFFLINE
-// when it was chosen offline; a de-duplicated v5 record carries the group field of its smallest handle.
+// Choose = false: every shared member passes through as a record of its own (group field = its group id); `g` is unused.
+// Choose = true: in a row's match list a shared member stands for its group only if it is the group's REPRESENTATIVE
+// (members[groups[g].off]); every other member entry is dropped.  Every matched filter node emits its whole value set, so the
+// representative appears once per appearance of the group.  Per appearance the warp scans the group's block and chooses; a
+// chosen v3 member is a direct record, a chosen v5 member joins the row's v5 relations and is de-duplicated per client with
+// them.  A chosen record's group field is the group id | GM_SUBREL_OFFLINE when it was chosen offline.
+// In both forms a de-duplicated v5 record carries the client's smallest handle and that handle's group field.  The choosing
+// form alone stages the group fields (s_grp): the expand form keeps 24 KiB of shared memory and its registers.
+// k_relations(p) is the expand form; k_relations_choose (below) names the choosing one.
+template <bool Choose = false>
 __global__ void __launch_bounds__(256)
-k_relations_choose(RelParams p, RelGroups g) {
-    __shared__ u32 s_key[8][REL_STAGE], s_h[8][REL_STAGE], s_sub[8][REL_STAGE], s_grp[8][REL_STAGE];
+k_relations(RelParams p, RelGroups g = RelGroups{}) {
+    __shared__ u32 s_key[8][REL_STAGE], s_h[8][REL_STAGE], s_sub[8][REL_STAGE], s_grp[8][Choose ? REL_STAGE : 1];
     const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5, lt = lanemask_lt();
     const u32 gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
     u32* sk = s_key[wid]; u32* sh = s_h[wid]; u32* ss = s_sub[wid]; u32* sg = s_grp[wid];
@@ -217,7 +129,8 @@ k_relations_choose(RelParams p, RelGroups g) {
         const uint2 sp = p.spans[t];
         const u32 off = sp.x, cnt = sp.y;
         const u32 pub = p.pubs ? p.pubs[t] : REL_NONE;
-        // classify one handle: 0 dropped, 1 direct (v3), 2 v5 relation subject to per-client de-dup, 3 a group's representative
+        // classify one handle: 0 dropped, 1 direct (v3, or a shared member passed through), 2 v5 relation subject to per-client
+        // de-dup, 3 a group's representative (choosing form)
         auto classify = [&](u32 i, u32& h, gm_rel& r) -> u32 {
             if (i >= cnt) return 0u;
             h = p.ids[off + i];
@@ -225,21 +138,23 @@ k_relations_choose(RelParams p, RelGroups g) {
             r = load_rel(p.rels + h);
             if (!(r.flags & GM_REL_LIVE)) return 0u;
             const u32 grp = r.flags >> 8;
-            if (grp) return grp < g.n_groups && g.groups[grp].y && g.members[g.groups[grp].x] == h ? 3u : 0u;   // no_local: in the choice
+            if constexpr (Choose) if (grp) return grp < g.n_groups && g.groups[grp].y && g.members[g.groups[grp].x] == h ? 3u : 0u;   // no_local: in the choice
             if ((r.flags & GM_REL_V5) && (r.flags & GM_REL_NO_LOCAL) && pub != REL_NONE && r.id_idx == pub) return 0u;   // router.rs:184-189
-            return (r.flags & GM_REL_V5) ? 2u : 1u;
+            return ((r.flags & GM_REL_V5) && grp == 0u) ? 2u : 1u;
         };
         // the choices of the representatives in one 32-entry chunk, in list order; f(handle, record, group field) per chosen member
         auto each_choice = [&](u32 i0, u32 c, u32 h, u32 grp, auto&& f) {
-            u32 bt = __ballot_sync(0xFFFFFFFFu, c == 3u);
-            while (bt) {
-                const u32 src = __ffs(bt) - 1; bt &= bt - 1;
-                const u32 rh = __shfl_sync(0xFFFFFFFFu, h, src), rg = __shfl_sync(0xFFFFFFFFu, grp, src), at = i0 + src;
-                u32 occ = 0;                                            // earlier appearances of the same representative
-                for (u32 j0 = 0; j0 < at; j0 += 32) occ += __popc(__ballot_sync(0xFFFFFFFFu, j0 + lane < at && p.ids[off + j0 + lane] == rh));
-                bool offline = false;
-                const u32 ch = share_choose(p, g, t, rg, occ, pub, lane, offline);
-                if (ch != REL_NONE) f(ch, load_rel(p.rels + ch), rg | (offline ? GM_SUBREL_OFFLINE : 0u));
+            if constexpr (Choose) {
+                u32 bt = __ballot_sync(0xFFFFFFFFu, c == 3u);
+                while (bt) {
+                    const u32 src = __ffs(bt) - 1; bt &= bt - 1;
+                    const u32 rh = __shfl_sync(0xFFFFFFFFu, h, src), rg = __shfl_sync(0xFFFFFFFFu, grp, src), at = i0 + src;
+                    u32 occ = 0;                                            // earlier appearances of the same representative
+                    for (u32 j0 = 0; j0 < at; j0 += 32) occ += __popc(__ballot_sync(0xFFFFFFFFu, j0 + lane < at && p.ids[off + j0 + lane] == rh));
+                    bool offline = false;
+                    const u32 ch = share_choose(p, g, t, rg, occ, pub, lane, offline);
+                    if (ch != REL_NONE) f(ch, load_rel(p.rels + ch), rg | (offline ? GM_SUBREL_OFFLINE : 0u));
+                }
             }
         };
         // ---- pass 1: count, choose, stage the v5 relations (chosen v5 members included) ----
@@ -249,7 +164,10 @@ k_relations_choose(RelParams p, RelGroups g) {
             const u32 c = classify(i0 + lane, h, r);
             ndirect += __popc(__ballot_sync(0xFFFFFFFFu, c == 1u));
             const u32 bv = __ballot_sync(0xFFFFFFFFu, c == 2u);
-            if (c == 2u) { const u32 at = nv + __popc(bv & lt); if (at < REL_STAGE) { sk[at] = r.client_key; sh[at] = h; ss[at] = r.sub_id; sg[at] = 0u; } }
+            if (c == 2u) {
+                const u32 at = nv + __popc(bv & lt);
+                if (at < REL_STAGE) { sk[at] = r.client_key; sh[at] = h; ss[at] = r.sub_id; if constexpr (Choose) sg[at] = 0u; }
+            }
             nv += __popc(bv);
             each_choice(i0, c, h, r.flags >> 8, [&](u32 ch, const gm_rel& cr, u32 gw) {
                 if (!(cr.flags & GM_REL_V5)) { ++ndirect; return; }
@@ -259,7 +177,8 @@ k_relations_choose(RelParams p, RelGroups g) {
         }
         __syncwarp();
         const bool overflow = nv > REL_STAGE;
-        // ---- de-dup: as k_relations ----
+        // ---- de-dup: entry e represents its client iff it holds the smallest handle of the client's relations (the same handle can
+        //      occur twice: a topic with a literal '+' / '#' level visits a wildcard child twice — ties go to the earlier entry) ----
         u32 nreps = 0, nsubs = 0;
         if (!overflow) {
             for (u32 e0 = 0; e0 < nv; e0 += 32) {
@@ -284,7 +203,7 @@ k_relations_choose(RelParams p, RelGroups g) {
         const bool fits = hb + total <= p.cap_rels && sb + nsubs <= p.cap_sub_ids && hb + total <= 0xFFFFFFFFull && sb + nsubs <= 0xFFFFFFFFull;
         if (lane == 0) { p.out_spans[t] = make_uint2(fits ? static_cast<u32>(hb) : 0u, total); if (overflow) p.status[t] = 1; }
         if (!fits || total == 0) { __syncwarp(); continue; }
-        // ---- pass 2: direct records (chosen v3 members, after an overflow every v5 relation too), then the v5 representatives.
+        // ---- pass 2: direct records (chosen v3 members; after an overflow every v5 relation too), then the v5 representatives.
         //      The choices are made again: they are a pure function of the row, the group and the appearance ----
         u32 w = 0;
         for (u32 i0 = 0; i0 < cnt; i0 += 32) {
@@ -292,7 +211,7 @@ k_relations_choose(RelParams p, RelGroups g) {
             const u32 c = classify(i0 + lane, h, r);
             const bool take = c == 1u || (overflow && c == 2u);
             const u32 b = __ballot_sync(0xFFFFFFFFu, take);
-            if (take) p.out_rels[hb + w + __popc(b & lt)] = gm_sub_relation{r.node_id, h, 0u, 0u, 0u};
+            if (take) p.out_rels[hb + w + __popc(b & lt)] = gm_sub_relation{r.node_id, h, r.flags >> 8, 0u, 0u};
             w += __popc(b);
             each_choice(i0, c, h, r.flags >> 8, [&](u32 ch, const gm_rel& cr, u32 gw) {
                 if ((cr.flags & GM_REL_V5) && !overflow) return;
@@ -315,15 +234,34 @@ k_relations_choose(RelParams p, RelGroups g) {
                 const u32 inc = warp_incl_scan(mys, lane);
                 if (rep) {
                     const u32 so = static_cast<u32>(sb) + ws + (inc - mys);
-                    p.out_rels[hb + w + __popc(br & lt)] = gm_sub_relation{load_rel(p.rels + h).node_id, h, sg[e], nsub ? so : 0u, nsub};
+                    p.out_rels[hb + w + __popc(br & lt)] = gm_sub_relation{load_rel(p.rels + h).node_id, h, Choose ? sg[e] : 0u, nsub ? so : 0u, nsub};
                     u32 k = 0;
-                    for (u32 j = 0; j < nv && k < nsub; ++j) if (sk[j] == key && ss[j] != 0u) p.out_sub_ids[so + k++] = ss[j];
+                    for (u32 j = 0; j < nv && k < nsub; ++j) if (sk[j] == key && ss[j] != 0u) p.out_sub_ids[so + k++] = ss[j];   // types.rs:497-503
                 }
                 w += __popc(br); ws += __shfl_sync(0xFFFFFFFFu, inc, 31);
             }
         }
         __syncwarp();
     }
+}
+
+constexpr auto k_relations_choose = k_relations<true>;
+
+// One launch of k_relations over the ABI's buffers (n >= 1): the expand form without a group table, the choosing form with
+// one.  One warp per topic, at most 8 CTAs per SM.  The caller zeroes o.d_needed first.
+inline void launch_relations(const gm_span* spans, const u32* ids, u64 n, const u32* pubs, const gm_rel* rels, u64 n_rels, const gm_rel_groups* gr,
+                             const gm_rel_out& o, int num_sms, cudaStream_t s) {
+    RelParams rp{};
+    rp.spans = reinterpret_cast<const uint2*>(spans); rp.ids = ids; rp.n = static_cast<u32>(n); rp.pubs = pubs;
+    rp.rels = rels; rp.n_rels = static_cast<u32>(n_rels);
+    rp.out_spans = reinterpret_cast<uint2*>(o.d_spans); rp.out_rels = o.d_rels; rp.cap_rels = o.cap_rels;
+    rp.out_sub_ids = o.d_sub_ids; rp.cap_sub_ids = o.cap_sub_ids;
+    rp.needed = reinterpret_cast<unsigned long long*>(o.d_needed); rp.status = o.d_status;
+    RelGroups rg{};
+    if (gr) { rg.groups = reinterpret_cast<const uint2*>(gr->d_groups); rg.n_groups = gr->n_groups; rg.members = gr->d_members; rg.online = gr->d_online; rg.n_online_bits = gr->n_online_bits; rg.seed = gr->seed; }
+    const unsigned grid = static_cast<unsigned>(std::min<u64>((n + 7) / 8, static_cast<u64>(num_sms) * 8));
+    if (gr) GM_LAUNCH(k_relations_choose, grid, 256, 0, s, rp, rg);
+    else GM_LAUNCH(k_relations, grid, 256, 0, s, rp);
 }
 
 }  // namespace gm

@@ -252,38 +252,20 @@ bool GpuRouter::filter(uint32_t fi, const std::string** name, std::vector<uint64
     return true;
 }
 
-// per-client de-dup of ONE topic on the host — only for topics the kernel flagged (more v5 relations than it stages)
-int32_t GpuRouter::host_dedup_topic(const gm_sub_relation* in, uint32_t cnt, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids) {
+// per-client de-dup of ONE topic on the host — only for topics the kernel flagged (more v5 relations than it stages).  A v5
+// relation joins the de-dup unless it is a shared member of the plain call (`chosen` false: every member passes through); as on
+// the device, the client's smallest handle represents it, with that record's group field, and the ids accumulate in list order.
+int32_t GpuRouter::host_dedup_topic(const gm_sub_relation* in, uint32_t cnt, bool chosen, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids) {
     struct V5Entry { size_t rel_pos; std::vector<uint32_t> ids; };
     std::unordered_map<uint32_t, V5Entry> v5;                 // client_key -> (its relation, accumulated ids)
     for (uint32_t k = 0; k < cnt; ++k) {
         const uint32_t h = in[k].handle;
         const gm_rel& d = rel_host_[h];
-        if (!(d.flags & GM_REL_V5) || (d.flags >> 8)) { rels.push_back(gm_sub_relation{d.node_id, h, d.flags >> 8, 0, 0}); continue; }
+        const gm_sub_relation sr{d.node_id, h, in[k].group, 0, 0};
+        if (!(d.flags & GM_REL_V5) || (!chosen && (d.flags >> 8))) { rels.push_back(sr); continue; }
         auto it = v5.find(d.client_key);
-        if (it == v5.end()) { V5Entry e{rels.size(), {}}; if (d.sub_id) e.ids.push_back(d.sub_id); rels.push_back(gm_sub_relation{d.node_id, h, 0, 0, 0}); v5.emplace(d.client_key, std::move(e)); }
-        else if (d.sub_id) it->second.ids.push_back(d.sub_id);
-    }
-    for (auto& kv : v5) {
-        gm_sub_relation& sr = rels[kv.second.rel_pos];
-        sr.sub_ids_off = static_cast<uint32_t>(sub_ids.size()); sr.sub_ids_cnt = static_cast<uint32_t>(kv.second.ids.size());
-        sub_ids.insert(sub_ids.end(), kv.second.ids.begin(), kv.second.ids.end());
-    }
-    return GM_OK;
-}
-
-// the same for a topic of the choosing form: chosen v5 members (group field set) are de-duplicated like any other v5 relation, and
-// the client's smallest handle represents it, as on the device
-int32_t GpuRouter::host_dedup_topic_chosen(const gm_sub_relation* in, uint32_t cnt, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids) {
-    struct V5Entry { size_t rel_pos; std::vector<uint32_t> ids; };
-    std::unordered_map<uint32_t, V5Entry> v5;
-    for (uint32_t k = 0; k < cnt; ++k) {
-        const uint32_t h = in[k].handle;
-        const gm_rel& d = rel_host_[h];
-        if (!(d.flags & GM_REL_V5)) { rels.push_back(gm_sub_relation{d.node_id, h, in[k].group, 0, 0}); continue; }
-        auto it = v5.find(d.client_key);
-        if (it == v5.end()) it = v5.emplace(d.client_key, V5Entry{rels.size(), {}}).first, rels.push_back(gm_sub_relation{d.node_id, h, in[k].group, 0, 0});
-        else if (h < rels[it->second.rel_pos].handle) rels[it->second.rel_pos] = gm_sub_relation{d.node_id, h, in[k].group, 0, 0};
+        if (it == v5.end()) { it = v5.emplace(d.client_key, V5Entry{rels.size(), {}}).first; rels.push_back(sr); }
+        else if (h < rels[it->second.rel_pos].handle) rels[it->second.rel_pos] = sr;
         if (d.sub_id) it->second.ids.push_back(d.sub_id);
     }
     for (auto& kv : v5) {
@@ -412,7 +394,7 @@ int32_t GpuRouter::matches_batch(const gm_id* publishers, const char* blob, cons
     for (uint64_t i = 0; i < n; ++i) {
         const size_t begin = rels.size();
         const uint32_t off = out_spans[i].off, cnt = out_spans[i].cnt;
-        if (status[i] == 1) { status[i] = 0; R_TRY(share_seed ? host_dedup_topic_chosen(dev.data() + off, cnt, rels, sub_ids) : host_dedup_topic(dev.data() + off, cnt, rels, sub_ids)); }
+        if (status[i] == 1) { status[i] = 0; R_TRY(host_dedup_topic(dev.data() + off, cnt, share_seed != nullptr, rels, sub_ids)); }
         else if (status[i] == 0)
             for (uint32_t k = 0; k < cnt; ++k) {
                 gm_sub_relation sr = dev[off + k];

@@ -12,8 +12,10 @@
 //             v5 per-client de-dup with accumulation of subscription identifiers (types.rs:488-506) -> the host only
 //             receives the finished gm_sub_relation records by DMA.  The router keeps a 24-byte gm_rel record per
 //             handle in HBM (shipped incrementally).  matches_batch returns every shared-group member; with a seed
-//             it chooses one per group on the device (k_relations_choose, subscribe.rs:66-104 with a seeded draw),
-//             from per-group member blocks and an online bitmap the router keeps in device layout.
+//             it chooses one per group on the device (k_relations<true>, subscribe.rs:66-104 with a seeded draw),
+//             from per-group member blocks and an online bitmap the router keeps in device layout.  A topic with more
+//             v5 relations than the kernel stages is de-duplicated by host_dedup_topic, by the kernel's rule: the
+//             client's smallest handle represents it.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -75,7 +77,7 @@ class GpuRouter {
     Dev d_rels_, d_blob_, d_offs_, d_spans_, d_status_, d_ids_, d_needed_, d_pubs_, d_ospans_, d_orels_, d_subs_;
     std::vector<uint32_t> pubs_;
     void* stream_ = nullptr;
-    // ---- shared groups in device layout (k_relations_choose): group id -> a block of live member handles with spare room in one
+    // ---- shared groups in device layout (k_relations<true>): group id -> a block of live member handles with spare room in one
     //      pool; a block that fills up moves to the pool's end, and the pool is re-packed once the abandoned blocks pass half of it.
     //      The header, the pool and the online bitmap are shipped by dirty range, like rel_host_.
     struct Dirty { uint32_t lo = 0xFFFFFFFFu, hi = 0; void mark(uint32_t a, uint32_t b) { lo = std::min(lo, a); hi = std::max(hi, b); } bool any() const { return hi > lo; } };
@@ -97,8 +99,7 @@ class GpuRouter {
     void member_remove(uint32_t handle);
     void repack_groups();
     int32_t ship_groups(void* stream);
-    int32_t host_dedup_topic(const gm_sub_relation* in, uint32_t cnt, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids);
-    int32_t host_dedup_topic_chosen(const gm_sub_relation* in, uint32_t cnt, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids);
+    int32_t host_dedup_topic(const gm_sub_relation* in, uint32_t cnt, bool chosen, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids);
 };
 
 }  // namespace gm

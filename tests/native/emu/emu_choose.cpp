@@ -1,11 +1,10 @@
-// TEST INFRASTRUCTURE: the shared-subscription choice (relations.cuh k_relations_choose, the kernel behind
-// gm_relations_choose_device) over HOST memory, on the CPU emulation in cuda_runtime.h.  Exposed as a small C interface for
+// TEST INFRASTRUCTURE: the shared-subscription choice (relations.cuh k_relations<true> through launch_relations, the launch
+// behind gm_relations_choose_device) over HOST memory, on the CPU emulation in cuda_runtime.h.  It builds from relations.cuh
+// alone, without the host tries of emu_driver.cpp.  Exposed as a small C interface for
 // tests/test_shared_choice_cpu.py, which compares the results with a Python model.  Build (the test does it):
 //   g++ -O1 -g -std=c++17 -DGM_CPU_EMU -Itests/native/emu -Irmqtt_b200/csrc -shared -fPIC -pthread tests/native/emu/emu_choose.cpp \
 //       -o <out>.so     (+ -fsanitize=address,undefined for the ASan run)
 #include <cuda_runtime.h>      // the emulation (this directory is first on the include path)
-
-#include <algorithm>
 
 #include "relations.cuh"
 
@@ -17,21 +16,15 @@ constexpr u32 EMU_SMS = 2;               // as the driver of the other kernels: 
 
 extern "C" {
 
-// gm_relations_choose_device over host arrays (k_relations_choose, engine.cu's grid); online = null: every client online
+// gm_relations_choose_device over host arrays; online = null: every client online
 int32_t emu_relations_choose(const gm_span* spans, const uint32_t* ids, uint64_t n, const uint32_t* pubs, const gm_rel* rels, uint64_t n_rels,
                              const gm_span* groups, uint32_t n_groups, const uint32_t* members, const uint32_t* online, uint32_t n_online_bits, uint64_t seed,
                              gm_span* out_spans, gm_sub_relation* out_rels, uint64_t cap_rels, uint32_t* out_sub_ids, uint64_t cap_sub_ids, uint64_t* needed3,
                              int32_t* status) {
     needed3[0] = needed3[1] = needed3[2] = 0;
     if (n == 0) return 0;
-    RelParams rp{};
-    rp.spans = reinterpret_cast<const uint2*>(spans); rp.ids = ids; rp.n = static_cast<u32>(n); rp.pubs = pubs; rp.rels = rels; rp.n_rels = static_cast<u32>(n_rels);
-    rp.out_spans = reinterpret_cast<uint2*>(out_spans); rp.out_rels = out_rels; rp.cap_rels = cap_rels; rp.out_sub_ids = out_sub_ids; rp.cap_sub_ids = cap_sub_ids;
-    rp.needed = reinterpret_cast<unsigned long long*>(needed3); rp.status = status;
-    RelGroups rg{};
-    rg.groups = reinterpret_cast<const uint2*>(groups); rg.n_groups = n_groups; rg.members = members; rg.online = online; rg.n_online_bits = n_online_bits; rg.seed = seed;
-    const unsigned grid = static_cast<unsigned>(std::min<u64>((n + 7) / 8, static_cast<u64>(EMU_SMS) * 8));
-    emu::launch(dim3(grid), dim3(256), [&] { k_relations_choose(rp, rg); });
+    const gm_rel_groups g{groups, n_groups, members, online, n_online_bits, seed};
+    launch_relations(spans, ids, n, pubs, rels, n_rels, &g, gm_rel_out{out_spans, out_rels, cap_rels, out_sub_ids, cap_sub_ids, needed3, status}, EMU_SMS, nullptr);
     return 0;
 }
 

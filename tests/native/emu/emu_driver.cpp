@@ -409,17 +409,12 @@ int32_t emu_retain_table(void* h, uint32_t which, const void** ptr, uint64_t* co
     return 0;
 }
 
-// gm_relations_expand_device over host arrays (k_relations)
+// gm_relations_expand_device over host arrays (k_relations<false>)
 int32_t emu_relations(const gm_span* spans, const uint32_t* ids, uint64_t n, const uint32_t* pubs, const gm_rel* rels, uint64_t n_rels, gm_span* out_spans,
                       gm_sub_relation* out_rels, uint64_t cap_rels, uint32_t* out_sub_ids, uint64_t cap_sub_ids, uint64_t* needed3, int32_t* status) {
     needed3[0] = needed3[1] = needed3[2] = 0;
     if (n == 0) return 0;
-    RelParams rp{};
-    rp.spans = reinterpret_cast<const uint2*>(spans); rp.ids = ids; rp.n = static_cast<u32>(n); rp.pubs = pubs; rp.rels = rels; rp.n_rels = static_cast<u32>(n_rels);
-    rp.out_spans = reinterpret_cast<uint2*>(out_spans); rp.out_rels = out_rels; rp.cap_rels = cap_rels; rp.out_sub_ids = out_sub_ids; rp.cap_sub_ids = cap_sub_ids;
-    rp.needed = reinterpret_cast<unsigned long long*>(needed3); rp.status = status;
-    const unsigned grid = static_cast<unsigned>(std::min<u64>((n + 7) / 8, static_cast<u64>(EMU_SMS) * 8));
-    emu::launch(dim3(grid), dim3(256), [&] { k_relations(rp); });
+    launch_relations(spans, ids, n, pubs, rels, n_rels, nullptr, gm_rel_out{out_spans, out_rels, cap_rels, out_sub_ids, cap_sub_ids, needed3, status}, EMU_SMS, nullptr);
     return 0;
 }
 

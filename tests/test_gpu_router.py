@@ -133,6 +133,28 @@ def test_v5_per_client_dedup_on_the_device_and_its_host_fallback(n_clients, per_
         assert sorted(lines) == want, t
 
 
+@pytest.mark.parametrize("shared", [False, True])
+def test_merged_v5_record_carries_the_smallest_handle(shared):
+    """A v5 client matched through several subscriptions gets the record of its smallest handle, from the device ("u/a/x": 10 v5
+    relations) and from the host fallback ("t/a/x": 600, more than the kernel stages), in gmr_matches_batch and
+    gmr_matches_batch_shared.  Every client subscribes to the filter the walk lists last first, so its first-listed handle is
+    not its smallest."""
+    r = GpuRouter()
+    sizes = {"t": 300, "u": 5}
+    for prefix, n_clients in sizes.items():
+        for c in range(n_clients):
+            for f in (f"{prefix}/a/x", f"{prefix}/#"):         # the walk lists "<prefix>/#" before "<prefix>/a/x"
+                r.add(f, Id(1, f"{prefix}{c}", c), SubscriptionOptions(qos=1, is_v5=True, sub_id=1 + c % 7))
+    handle = {r._relation(h): h for h in range(2 * sum(sizes.values()))}
+    got = r.matches_batch(["t/a/x", "u/a/x"], seed=7 if shared else None)
+    for (prefix, n_clients), rels in zip(sizes.items(), got):
+        assert sorted(x.client_id for x in rels) == sorted(f"{prefix}{c}" for c in range(n_clients))
+        for x in rels:
+            c = int(x.client_id[1:])
+            assert x.sub_ids == [1 + c % 7] * 2
+            assert handle[(x.topic_filter, x.client_id)] == min(handle[(f, x.client_id)] for f in (f"{prefix}/a/x", f"{prefix}/#")), x
+
+
 def test_secondary_readers_through_descriptor_mode():
     """_has_matches / _get_routes / Router::get (router.rs:139-158, 522-546) answered by the engine (descriptor mode: one
     descriptor per matched filter), against the oracle's restatement — no second CPU trie."""

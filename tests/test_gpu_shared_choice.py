@@ -180,6 +180,63 @@ def test_literal_plus_topic_gets_two_choices():
         assert len(got[0]) == 2 and len(got[1]) == 1
 
 
+def _plain_want(P, topic, pub):
+    """gmr_matches_batch restated on the same relations: every shared member passes through as a line of its own."""
+    lines, v5 = [], {}
+    for fi in P.o.tree.matches(topic):
+        filt = P.o.filters[fi]
+        for client, (node, tag, is_v5, no_local, sub_id, group) in P.o.rel.get(filt, {}).items():
+            if is_v5 and no_local and (pub.node_id, pub.client_id, pub.tag) == (node, client, tag):
+                continue
+            if group:
+                lines.append(f"g|{node}|{filt}|{group}|{client}")
+            elif is_v5:
+                v5.setdefault((node, client), []).extend([sub_id] if sub_id else [])
+            else:
+                lines.append(f"3|{node}|{filt}|{client}")
+    lines += [f"5|{node}|{client}|" + ",".join(map(str, sorted(ids))) for (node, client), ids in v5.items()]
+    return sorted(lines)
+
+
+def _plain_lines(P, rels):
+    lines = []
+    for x in rels:
+        if x.group:
+            assert not x.sub_ids
+            lines.append(f"g|{x.node_id}|{x.topic_filter}|{P.r.group_members(x.group)[1]}|{x.client_id}")
+        elif P.opts[(x.topic_filter, x.client_id)][1].is_v5:
+            lines.append(f"5|{x.node_id}|{x.client_id}|" + ",".join(map(str, sorted(x.sub_ids))))
+        else:
+            lines.append(f"3|{x.node_id}|{x.topic_filter}|{x.client_id}")
+    return sorted(lines)
+
+
+def test_flagged_topics_finished_on_the_host():
+    """Topics with more v5 relations than the kernel stages (256) are de-duplicated on the host: chosen v5 members (many of them
+    clients with a plain v5 relation too), v3 group members, no_local drops and plain v5 relations, against the restatement.
+    gmr_matches_batch on the same topics passes every member through, unmerged."""
+    rng = random.Random(13)
+    P = Pair()
+    for k in range(300):                                     # 300 plain v5 relations on every "h/..." topic
+        P.add("h/#", Id(1 + k % 2, f"p{k}", k), SubscriptionOptions(qos=1, is_v5=True, no_local=k % 5 == 0, sub_id=rng.choice([0, 3, 5, 9])))
+    for k in range(0, 300, 3):                               # v5 members; the even ones are plain v5 clients as well
+        P.add("h/+/x", Id(1 + k % 2, f"p{k}" if k % 2 == 0 else f"m{k}", k),
+              SubscriptionOptions(qos=1, is_v5=True, no_local=k % 4 == 0, sub_id=rng.choice([0, 4, 7]), shared_group=f"v{k % 4}"))
+    for k in range(40):
+        P.add("h/a/+", Id(2, f"s{k}", k), SubscriptionOptions(shared_group=f"w{k % 3}"))
+    for k in range(20):
+        P.add("h/+/+", Id(1, f"d{k}", k))
+    for k in range(0, 300, 7):
+        P.set_online(Id(1 + k % 2, f"p{k}"), False)
+    topics = ["h/a/x", "h/b/x", "h/a/y", "h/+/x", "q/a"]
+    pubs = [Id(1, "p0", 0), Id(1, "p12", 12), Id(2, "s1", 1), Id(9, "nobody"), Id(1, "p20", 20)]
+    for seed in range(6):
+        P.check(topics, pubs, seed)
+    plain = P.r.matches_batch(topics, pubs)
+    for row, (t, p) in enumerate(zip(topics, pubs)):
+        assert _plain_lines(P, plain[row]) == _plain_want(P, t, p), t
+
+
 def _raw_shared(P, topics, seed, cap_rels, cap_subs=1 << 16):
     blob, offs = pack(topics)
     n = len(topics)

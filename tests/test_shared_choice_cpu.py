@@ -1,4 +1,4 @@
-"""CPU tier of the shared-subscription choice (relations.cuh k_relations_choose, include/gpumqtt.h gm_relations_choose_device):
+"""CPU tier of the shared-subscription choice (relations.cuh k_relations<true>, include/gpumqtt.h gm_relations_choose_device):
 the key of the draw against two independent restatements, and the kernel, run on the CPU emulation (tests/native/emu/emu_choose.cpp), against a direct Python
 model, topic by topic — also under AddressSanitizer + UBSan."""
 import ctypes as C
@@ -283,7 +283,7 @@ def check_choice_kernel(lib):
 
 
 def test_choice_kernel_against_a_python_model(emu):
-    """k_relations_choose on the emulator equals the model topic by topic: groups of 1 to 1000 members, representatives twice,
+    """k_relations<true> on the emulator equals the model topic by topic: groups of 1 to 1000 members, representatives twice,
     dead / out-of-range handles and group ids, no_local (a group whose only member is the publisher), an offline group and a
     NULL bitmap, chosen v5 members merging with the same client's v5 relations, and the > 256 hand-over with status 1."""
     case = check_choice_kernel(emu)
