@@ -438,7 +438,7 @@ struct gm_engine {
         CUDA_TRY(ev);
         CUDA_TRY(cudaGetLastError());
         if (a.timing) ring_n++;
-        launches += 5;
+        launches += a.desc ? 5 : 6;
         if (a.d_needed) CUDA_TRY(cudaMemcpyAsync(a.d_needed, &m.ctrl->cursor, sizeof(u64), cudaMemcpyDeviceToDevice, s));
         if (!small) { CUDA_TRY(cudaEventRecord(c.ev_done, s)); c.recorded = true; }
         return GM_OK;
@@ -831,7 +831,7 @@ static int small_graph_match(gm_engine* e, MatchCtx& c, std::unique_lock<std::mu
     CUDA_TRY(cudaGraphLaunch(g->exec, c.sc));
     CUDA_TRY(cudaEventRecord(c.ev_done, c.sc));
     c.recorded = true;
-    e->launches += 5;
+    e->launches += desc ? 5 : 6;
     gd.unlock();
     CUDA_TRY(cudaEventSynchronize(c.ev_done));
     const u64 total = *reinterpret_cast<const u64*>(g->h_out);

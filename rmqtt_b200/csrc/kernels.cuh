@@ -4,8 +4,8 @@
 //                  validate, and intern every level through the device dictionary -> u32 tokens.
 //   k_match_fast   TopicTree::matches (rmqtt/src/trie.rs:299-347, MatchedIter::prepare): one topic per
 //                  thread walks the trie depth-first (one 32-byte load per visited node), then the warp
-//                  publishes its 32 match lists with a scan + load-balanced (ballot/shuffle) expansion:
-//                  single pass, per-topic contiguous output.
+//                  reserves its 32 match lists (per-topic contiguous output) and records their value sets.
+//   k_match_expand writes the ids of those value sets with a load-balanced (scan / shuffle search) copy.
 //   k_match_slow   the same walk for the topics the fast path defers (more levels than the fast
 //                  path stages in shared memory, or more matches than its staging pool): one warp per
 //                  topic, count pass + write pass, warp-cooperative value-range copies.
@@ -46,8 +46,8 @@ struct MatchParams {
     const u32* tok8_sorted;   // [n][8] token rows copied into locality order (MP_SORTED_ROWS)
     const u32* meta_sorted;   // [n]
     u32 tile_chunk;           // tiles a CTA takes from the global counter at once (<= 1: one tile per warp per grab)
-    // FUSED GATHER (peer memory): the publish phase writes every result DIRECTLY into the gathered buffers of all ranks
-    // (own included) over NVLink — no separate collective, the transfer overlaps the walk tile by tile.  Rank r's rows
+    // FUSED GATHER (peer memory): the match writes every result DIRECTLY into the gathered buffers of all ranks (own
+    // included) over NVLink — no separate collective; spans and indices as the walk goes, ids from k_match_expand.  Rank r's rows
     // occupy the fixed slab [r * slab_topics, ...) / ids [r * slab_ids, ...) of every rank's buffers.
     u32* g_ids[8];            // gathered id arrays of ranks 0..g_world-1 (peer pointers, CUDA IPC)
     uint2* g_spans[8];
@@ -60,8 +60,16 @@ struct MatchParams {
     const u32* n_ptr;         // small-batch graphs: the real batch size lives in device memory (n is then the capacity = row stride of `tok`)
     uint2* out_desc;          // DESCRIPTOR mode: matched value sets (ref, cnt16) per topic instead of expanded ids; spans index this array
     int* status;              // [n] per-topic status (k_tokenize wrote it); the deferred kernel reports GM_ERR_INTERNAL here
+    // ids mode: k_match_fast stores the matched value sets (ref, cnt) of every tile whose ids fit into `items`, in the order of
+    // their ids, and one record per tile; k_match_expand turns them into ids
+    uint2* items;
+    struct TileRec* tiles;    // [ceil(n / 32)], indexed by tile
+    unsigned long long* item_cursor;   // bump allocator over `items`
 };
-constexpr u32 MP_DIAG_NO_PUBLISH = 2u;   // diagnostics only: skip the publish phase
+// where k_match_expand finds a tile's value sets and writes its ids (n_items = 0: nothing to write)
+struct TileRec { u32 item_base, n_items; unsigned long long id_base; };
+static_assert(sizeof(TileRec) == 16, "one 16-byte record per tile");
+constexpr u32 MP_DIAG_NO_PUBLISH = 2u;   // diagnostics only: no ids are written (k_match_fast records no value sets for k_match_expand)
 constexpr u32 MP_SORTED_ROWS = 1u;   // k_bucket_scatter also copies token rows + meta into sorted order (coalesced reads in k_match_fast)
 constexpr u32 MAX_BUCKET_BITS = 18;   // locality buckets: 2^bits, bits = site_bits + sub_bits (engine.cu)
 constexpr u32 TOK8 = 8;              // levels kept in the per-topic 32-byte token row
@@ -415,6 +423,19 @@ __device__ __forceinline__ u32 next_tile_chunked(unsigned long long* s_chunk, u3
 // A matched value set waiting to be expanded into the output: values[ref .. ref+cnt) (or ref itself).
 struct Desc { u32 ref, cnt; };
 
+// Load-balanced expansion of a warp's 32 runs laid end to end (run lengths scanned into `exc`, the exclusive prefix): the
+// lane whose run holds flat index e, by binary search over `exc` — the last lane whose run starts at or before e (an
+// empty run starts where the next one does, so it never owns an index below the total).
+__device__ __forceinline__ u32 warp_run_owner(u32 exc, u32 e) {
+    u32 lo = 0;
+#pragma unroll
+    for (int step = 16; step; step >>= 1) {
+        const u32 v = __shfl_sync(0xFFFFFFFFu, exc, lo + step);
+        if (v <= e) lo += step;
+    }
+    return lo;
+}
+
 // K2: TopicTree::matches, one topic per thread (depth-first), one tile of 32 topics per warp.
 //
 //   walk     every thread follows its own topic down the trie: at a node it records the matched value
@@ -423,9 +444,10 @@ struct Desc { u32 ref, cnt; };
 //            child with ONE 32-byte load; when the literal path ends it resumes the deepest parked
 //            '+' child.  The dependent chain of a thread is one load long per visited node; latency is
 //            hidden by the other ~1.5 K resident threads of the SM.
-//   publish  warp-cooperative: per-lane totals -> warp scan -> one atomic reservation per tile ->
-//            load-balanced expansion of the descriptors (ballot/scan + binary search by shuffle) so
-//            that the id copies out of `values` and into out_ids are coalesced runs.
+//   publish  warp-cooperative: per-lane totals -> warp scan -> one atomic reservation of the tile's ids ->
+//            the tile's descriptors, lane-major, into the item array and one TileRec per tile.  The ids
+//            themselves are written by k_match_expand: expanding them here kept each warp away from the
+//            walk for a long serial chain of shuffles and scattered stores, and the walk is latency bound.
 //
 // (A warp-shared ballot-compacted frontier queue instead is bound by its collective overhead, not by memory.)
 // DESC = descriptor mode: the publish phase writes each topic's matched value-set references (ref, cnt16) — 8 bytes per
@@ -583,62 +605,29 @@ k_match_fast(MatchParams p, Desc* __restrict__ dpool, u32 pool_rows) {
                 for (u32 w = 0; w < p.g_world; ++w) { p.g_spans[w][p.g_base_topics + t] = gsp; p.g_index[w][p.g_base_topics + t] = gi; }
             } else p.spans[t] = make_uint2(fits ? static_cast<u32>(base + pre) : 0u, mine);
         }
-        const u32 maxd = __reduce_max_sync(0xFFFFFFFFu, nd);
+        auto store_descs = [&](uint2* __restrict__ outd) {     // this lane's nd descriptors, contiguous from outd
+            for (u32 k = 0; k < nd; ++k) {
+                uint2 v;
+                if (k < SD) v = s_desc[k][tid];
+                else { const Desc dd = dpool[static_cast<size_t>(k - SD) * nthreads + gtid]; v = make_uint2(dd.ref, dd.cnt); }
+                __stcs(outd + k, v);
+            }
+        };
         if (DESC) {
-            if (fits && wtotal) {
-                uint2* __restrict__ outd = p.out_desc + base + pre;     // this topic's descriptors, contiguous
-                for (u32 k = 0; k < nd; ++k) {
-                    uint2 v;
-                    if (k < SD) v = s_desc[k][tid];
-                    else { const Desc dd = dpool[static_cast<size_t>(k - SD) * nthreads + gtid]; v = make_uint2(dd.ref, dd.cnt); }
-                    __stcs(outd + k, v);
-                }
-            }
-        } else if (fits && wtotal && !(p.flags & MP_DIAG_NO_PUBLISH)) {
-            u32* __restrict__ out = p.out_ids + base;
-            u32 cur = pre;                                    // this lane's write position inside the tile chunk
-            for (u32 k = 0; k < maxd; ++k) {                  // row k: the k-th descriptor of every lane
-                Desc dsc{0u, 0u};
-                if (k < nd) {
-                    if (k < SD) { const uint2 v = s_desc[k][tid]; dsc = Desc{v.x, v.y}; }
-                    else dsc = dpool[static_cast<size_t>(k - SD) * nthreads + gtid];
-                }
-                const u32 ni = dsc.cnt;
-                const u32 dst = cur;
-                cur += ni;
-                // load-balanced expansion: flat id index e -> (owner lane, k) by binary search over `exc`.
-                // (one cooperative copy per large set + per-lane copies of the small ones is slower: the serial
-                //  shuffle/copy chain per set costs more than the search.)
-                u32 sc = ni;
+            if (fits && wtotal) store_descs(p.out_desc + base + pre);     // this topic's descriptors, contiguous
+        } else {
+            // the same descriptors, lane-major (the order of their ids in out_ids), for k_match_expand — only for a tile whose
+            // ids fit, so that k_match_expand writes only inside out_ids (see plan_match)
+            const u32 ni = (fits && !(p.flags & MP_DIAG_NO_PUBLISH)) ? nd : 0u;
+            u32 iinc = ni;
 #pragma unroll
-                for (int o = 1; o < 32; o <<= 1) { u32 v = __shfl_up_sync(0xFFFFFFFFu, sc, o); if (lane >= o) sc += v; }
-                const u32 tot = __shfl_sync(0xFFFFFFFFu, sc, 31);
-                const u32 exc = sc - ni;
-                // flat index e of the row -> owner lane by binary search over `exc`; with owner o: output position = e +
-                // (dst_o - exc_o), source index = e + (ref_o - exc_o); a single-value set has e == exc_o, so its value
-                // ref_o = e + (ref_o - exc_o) too — two broadcasts per element instead of four
-                const u32 delta = dst - exc, gamma = dsc.ref - exc;
-                const u32 single = __ballot_sync(0xFFFFFFFFu, ni == 1u);
-                for (u32 e0 = 0; e0 < tot; e0 += 32) {
-                    const u32 e = e0 + lane;
-                    u32 lo = 0;
-#pragma unroll
-                    for (int step = 16; step; step >>= 1) {
-                        u32 v = __shfl_sync(0xFFFFFFFFu, exc, lo + step);
-                        if (v <= e) lo += step;
-                    }
-                    const u32 o_delta = __shfl_sync(0xFFFFFFFFu, delta, lo);
-                    const u32 o_gamma = __shfl_sync(0xFFFFFFFFu, gamma, lo);
-                    if (e < tot) {
-                        const u32 src = e + o_gamma;
-                        const u32 val = ((single >> lo) & 1u) ? src : tv.values[src];
-                        if (GATHER) {        // posted stores into every rank's gathered array (NVLink for the peers)
-                            const unsigned long long at = p.g_base_ids + base + e + o_delta;
-                            for (u32 w = 0; w < p.g_world; ++w) p.g_ids[w][at] = val;
-                        } else __stcs(out + e + o_delta, val);   // streaming store: written once
-                    }
-                }
-            }
+            for (int o = 1; o < 32; o <<= 1) { u32 v = __shfl_up_sync(0xFFFFFFFFu, iinc, o); if (lane >= o) iinc += v; }
+            const u32 witems = __shfl_sync(0xFFFFFFFFu, iinc, 31);
+            u32 ibase = 0;      // (items stay below cap_ids <= 2^32 - 1)
+            if (lane == 0 && witems) ibase = static_cast<u32>(atomicAdd(p.item_cursor, static_cast<unsigned long long>(witems)));
+            ibase = __shfl_sync(0xFFFFFFFFu, ibase, 0);
+            if (lane == 0) p.tiles[tile] = TileRec{ibase, witems, base};
+            if (ni) store_descs(p.items + ibase + (iinc - ni));
         }
         const bool deferred = in_range && defer;
         u32 db = __ballot_sync(0xFFFFFFFFu, deferred);
@@ -656,6 +645,46 @@ k_match_fast(MatchParams p, Desc* __restrict__ dpool, u32 pool_rows) {
             sF += __shfl_xor_sync(0xFFFFFFFFu, sF, o); sM += __shfl_xor_sync(0xFFFFFFFFu, sM, o);
         }
         if (lane == 0) { atomicAdd(p.stats + 0, sV); atomicAdd(p.stats + 1, sE); atomicAdd(p.stats + 2, sF); atomicAdd(p.stats + 3, sM); }
+    }
+}
+
+// K2b: the ids of k_match_fast's tiles.  One warp per tile record; the tile's value sets (ref, cnt) are in id order and
+// are taken 32 at a time: warp scan of cnt, then every lane finds the set of its flat index (warp_run_owner) and copies one
+// id, so each 32-id step is one contiguous 128-byte run of out_ids.  GATHER: the ids go into the gathered array of every
+// rank in g_ids (push form: the own block only).
+template <bool GATHER>
+__global__ void __launch_bounds__(256)
+k_match_expand(MatchParams p) {
+    const u32 lane = threadIdx.x & 31;
+    const u32 gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+    const u32 n_act = p.n_ptr ? min(p.n, *p.n_ptr) : p.n;
+    const u32 ntiles = (n_act + 31) >> 5;
+    for (u32 tile = gwarp; tile < ntiles; tile += nwarps) {
+        const TileRec rec = p.tiles[tile];
+        unsigned long long at = (GATHER ? p.g_base_ids : 0ull) + rec.id_base;
+        for (u32 i0 = 0; i0 < rec.n_items; i0 += 32) {
+            const u32 i = i0 + lane;
+            const uint2 d = i < rec.n_items ? __ldcs(p.items + rec.item_base + i) : make_uint2(0u, 0u);
+            u32 sc = d.y;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { u32 v = __shfl_up_sync(0xFFFFFFFFu, sc, o); if (lane >= o) sc += v; }
+            const u32 tot = __shfl_sync(0xFFFFFFFFu, sc, 31);
+            const u32 exc = sc - d.y;
+            // with owner o: source index = e + (ref_o - exc_o); a one-value set has e == exc_o, so its value ref_o is that too
+            const u32 gamma = d.x - exc;
+            const u32 single = __ballot_sync(0xFFFFFFFFu, d.y == 1u);
+            for (u32 e0 = 0; e0 < tot; e0 += 32) {
+                const u32 e = e0 + lane;
+                const u32 o = warp_run_owner(exc, e);
+                const u32 src = e + __shfl_sync(0xFFFFFFFFu, gamma, o);
+                if (e < tot) {
+                    const u32 val = ((single >> o) & 1u) ? src : p.tv.values[src];
+                    if (GATHER) { for (u32 w = 0; w < p.g_world; ++w) p.g_ids[w][at + e] = val; }   // posted stores, NVLink for the peers
+                    else __stcs(p.out_ids + at + e, val);                                          // streaming store: written once
+                }
+            }
+            at += tot;
+        }
     }
 }
 

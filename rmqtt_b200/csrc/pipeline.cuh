@@ -15,7 +15,9 @@
 namespace gm {
 
 // ---- control blocks ----------------------------------------------------------------------------------------------------
-struct Ctrl { unsigned long long cursor; unsigned long long stats[24]; u32 slow_count; u32 tile_counter; };   // match control block, zeroed before every match
+// match control block, zeroed before every match (a pipelined host call keeps `cursor` across its chunks and clears the rest,
+// item_cursor included: every chunk has its own item array)
+struct Ctrl { unsigned long long cursor; unsigned long long item_cursor; unsigned long long stats[24]; u32 slow_count; u32 tile_counter; };
 
 // Retained-lookup control block.  counts[(depth + 3) * RQ] (tasks queued per round and queue slice; round 0 = k_retain_init)
 // and claim[depth + 3] (the task hand-out of every round) follow it in the same allocation.
@@ -54,7 +56,7 @@ inline size_t tok_bytes(u32 tok_levels, u32 n) { return tok_levels > TOK8 ? stat
 // capacity of n rows while the real batch size is read from `hdr` at run time; its fast and deferred grids are capped to n rows.
 struct MatchPlan {
     u32 n, tok_levels, nbuckets, stack_cap, pool_rows;
-    int tok_grid, scatter_grid, k2_grid, k3_blocks;
+    int tok_grid, scatter_grid, k2_grid, expand_grid, k3_blocks;
     size_t tok, tok8, meta, slow, ctrl, sort, hist, gstack, gpool;
 };
 inline MatchPlan plan_match(u32 n, u32 max_depth, const MatchKnobs& kn, int num_sms, bool small) {
@@ -68,10 +70,15 @@ inline MatchPlan plan_match(u32 n, u32 max_depth, const MatchKnobs& kn, int num_
     p.tok_grid = static_cast<int>((n + TOK_THREADS - 1) / TOK_THREADS);
     p.scatter_grid = static_cast<int>((n + 255) / 256);
     p.k2_grid = small ? std::max(1, std::min<int>(num_sms * k2_ctas, (n + K2_THREADS - 1) / K2_THREADS)) : num_sms * k2_ctas;
+    p.expand_grid = small ? std::max(1, std::min<int>(num_sms * 8, (n + 255) / 256)) : num_sms * 8;   // 8 warps of 256 threads, one tile each
     p.k3_blocks = small ? std::max(1, std::min<int>(num_sms, (n + 7) / 8)) : num_sms * 4;
     p.tok = tok_bytes(p.tok_levels, n); p.tok8 = static_cast<size_t>(n) * TOK8 * sizeof(u32);
     p.meta = p.slow = n * sizeof(u32); p.ctrl = sizeof(Ctrl);
-    p.sort = static_cast<size_t>(n) * 11 * sizeof(u32) + 64;        // carved in launch_match
+    // carved in launch_match: the locality order and sorted rows, then k_match_fast's tile records and value sets (ids mode).
+    // Only a tile whose ids fit stores its value sets, and a topic with more than K2_SMEM_DESCS + K2_POOL_ROWS (32) of them
+    // is deferred: at most 32 per row, whatever the output's capacity.  (Storing them only for tiles that fit also keeps
+    // k_match_expand inside the output: every set has at least one id, and those tiles' ids are disjoint ranges below cap_ids.)
+    p.sort = static_cast<size_t>(n) * 11 * sizeof(u32) + 64 + static_cast<size_t>((n + 31) / 32) * sizeof(TileRec) + 32ull * n * sizeof(uint2);
     p.hist = 2 * static_cast<size_t>(p.nbuckets) * sizeof(u32);     // counts[nbuckets] | cursor[nbuckets]
     p.gstack = static_cast<size_t>(num_sms) * 4 * 8 * p.stack_cap * sizeof(u64);
     p.gpool = static_cast<size_t>(num_sms) * k2_ctas * K2_THREADS * p.pool_rows * sizeof(Desc);
@@ -139,15 +146,18 @@ struct MatchIO {
 
 struct NoHook { void operator()(int) const {} };
 
-// k_tokenize -> k_bucket_scan -> k_bucket_scatter -> k_match_fast -> k_match_slow.  `at(k)` runs before the tokeniser (0), after
-// the locality pass (1), after the fast kernel (2) and after the deferred kernel (3).
+// k_tokenize -> k_bucket_scan -> k_bucket_scatter -> k_match_fast -> k_match_expand (ids only) -> k_match_slow.  `at(k)` runs
+// before the tokeniser (0), after the locality pass (1), after the fast kernel and the expansion (2) and after the deferred
+// kernel (3).
 template <class Hook = NoHook>
 inline void launch_match(const MatchPlan& p, const MatchScratch& m, const MatchIO& io, const MatchKnobs& kn, const TrieView& tv, cudaStream_t s, Hook at = {}) {
     const u32 n = p.n;
-    u32* bkey = m.sort;            // sort: bkey[n] | perm[n] | meta_sorted[n] | padding to 32 bytes | tok8_sorted[n][8]
+    u32* bkey = m.sort;            // sort: bkey[n] | perm[n] | meta_sorted[n] | padding to 32 bytes | tok8_sorted[n][8] | tiles | items
     u32* perm = bkey + n;
     u32* meta_sorted = perm + n;
     u32* tok8_sorted = meta_sorted + n + ((8 - (3 * static_cast<size_t>(n)) % 8) % 8);   // 32-byte aligned rows
+    TileRec* tiles = reinterpret_cast<TileRec*>(tok8_sorted + static_cast<size_t>(n) * TOK8);  // ... then tile records | value sets
+    uint2* items = reinterpret_cast<uint2*>(tiles + (n + 31) / 32);
     u32* bcursor = m.hist + p.nbuckets;
     at(0);
     auto k1 = kn.tok_bulk ? k_tokenize<true> : k_tokenize<false>;
@@ -160,6 +170,7 @@ inline void launch_match(const MatchPlan& p, const MatchScratch& m, const MatchI
     mp.tv = tv; mp.tok8 = m.tok8; mp.tok = m.tok; mp.meta = m.meta; mp.n = n; mp.n_ptr = io.hdr; mp.tok_levels = p.tok_levels;
     mp.spans = reinterpret_cast<uint2*>(io.spans); mp.out_ids = static_cast<u32*>(io.out); mp.out_desc = static_cast<uint2*>(io.out); mp.cap_ids = io.cap;
     mp.status = io.status;
+    mp.items = items; mp.tiles = tiles; mp.item_cursor = &m.ctrl->item_cursor;
     mp.trees = io.trees;
     mp.cursor = &m.ctrl->cursor; mp.slow_list = m.slow; mp.slow_count = &m.ctrl->slow_count;
     mp.tile_counter = &m.ctrl->tile_counter; mp.stats = m.ctrl->stats;
@@ -179,6 +190,10 @@ inline void launch_match(const MatchPlan& p, const MatchScratch& m, const MatchI
     const bool gather = io.gather != nullptr;
     auto k2 = k2_kernel(io.stats, io.desc, gather);
     GM_LAUNCH(k2, p.k2_grid, K2_THREADS, K2_SMEM, s, mp, m.gpool, p.pool_rows);
+    if (!io.desc) {
+        auto kx = gather ? k_match_expand<true> : k_match_expand<false>;
+        GM_LAUNCH(kx, p.expand_grid, 256, 0, s, mp);
+    }
     at(2);
     auto k3 = k3_kernel(io.stats, io.desc, gather);
     GM_LAUNCH(k3, p.k3_blocks, 256, 0, s, mp, m.gstack, p.stack_cap);

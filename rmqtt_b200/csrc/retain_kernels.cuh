@@ -355,12 +355,7 @@ k_retain_expand(const RDesc* __restrict__ descs, const u32* __restrict__ n_desc_
         const u32 exc = sc - ni;
         for (u32 e0 = 0; e0 < tot; e0 += 32) {
             const u32 e = e0 + lane;
-            u32 lo = 0;
-#pragma unroll
-            for (int step = 16; step; step >>= 1) {
-                u32 x = __shfl_sync(0xFFFFFFFFu, exc, lo + step);
-                if (x <= e) lo += step;
-            }
+            const u32 lo = warp_run_owner(exc, e);
             const u32 o_exc = __shfl_sync(0xFFFFFFFFu, exc, lo);
             const u32 o_ref = __shfl_sync(0xFFFFFFFFu, d.ref, lo);
             const u32 o_kind = __shfl_sync(0xFFFFFFFFu, d.kind, lo);

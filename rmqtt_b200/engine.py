@@ -436,7 +436,11 @@ class Engine:
         self._check(self._lib.gm_debug_knob(self._h, name.encode(), int(value)))
 
     def kernel_ms(self, max_calls: int = 64) -> np.ndarray:
-        """[calls, 3] device milliseconds (tokenise, match, deferred) of the last match calls, oldest first."""
+        """[calls, 3] device milliseconds (tokenise, match, deferred) of the last match calls, oldest first.
+
+        Column 0 is k_tokenize + k_bucket_scan + k_bucket_scatter.  Column 1 is k_match_fast plus, in ids mode,
+        k_match_expand, which writes the ids: a roofline that counts the id writes among the match's bytes divides
+        them by this column, so the expansion's time belongs in it.  Column 2 is k_match_slow."""
         out = np.zeros((max_calls, 3), dtype=np.float32)
         n = C.c_uint32(0)
         self._check(self._lib.gm_kernel_ms_ring(self._h, _vp(out), max_calls, C.byref(n)))
