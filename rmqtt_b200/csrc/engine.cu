@@ -426,12 +426,10 @@ struct gm_engine {
             CUDA_TRY(cudaStreamWaitEvent(s, ev_flush, 0));
             if (c.recorded) CUDA_TRY(cudaStreamWaitEvent(s, c.ev_done, 0));   // this context's scratch: one match at a time
         }
-        if (a.keep_cursor) CUDA_TRY(cudaMemsetAsync(static_cast<char*>(c.d_ctrl.p) + sizeof(unsigned long long), 0, sizeof(Ctrl) - sizeof(unsigned long long), s));
-        else CUDA_TRY(cudaMemsetAsync(c.d_ctrl.p, 0, sizeof(Ctrl), s));
-        CUDA_TRY(cudaMemsetAsync(c.d_hist.p, 0, p.nbuckets * sizeof(u32), s));
         MatchScratch m{};
         m.tok = c.d_tok.as<u32>(); m.tok8 = c.d_tok8.as<u32>(); m.meta = c.d_meta.as<u32>(); m.slow = c.d_slow.as<u32>(); m.sort = c.d_sort.as<u32>(); m.hist = c.d_hist.as<u32>();
         m.ctrl = c.d_ctrl.as<Ctrl>(); m.gstack = c.d_gstack.as<u64>(); m.gpool = c.d_gpool.as<Desc>();
+        for (const ByteRange& r : match_resets(p, m, a.keep_cursor).r) CUDA_TRY(cudaMemsetAsync(r.p, 0, r.bytes, s));
         cudaEvent_t* ev_t = ev_ring[ring_n % RING];
         cudaError_t ev = cudaSuccess;
         launch_match(p, m, a, kn, dev_view, s, [&](int k) { if (a.timing && ev == cudaSuccess) ev = cudaEventRecord(ev_t[k], s); });

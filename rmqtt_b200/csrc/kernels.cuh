@@ -69,7 +69,7 @@ struct MatchParams {
 // where k_match_expand finds a tile's value sets and writes its ids (n_items = 0: nothing to write)
 struct TileRec { u32 item_base, n_items; unsigned long long id_base; };
 static_assert(sizeof(TileRec) == 16, "one 16-byte record per tile");
-constexpr u32 MP_DIAG_NO_PUBLISH = 2u;   // diagnostics only: no ids are written (k_match_fast records no value sets for k_match_expand)
+constexpr u32 MP_DIAG_NO_PUBLISH = 2u;   // diagnostics only: the fast path writes no ids (k_match_fast records no value sets for k_match_expand; k_match_slow still writes the deferred topics' ids)
 constexpr u32 MP_SORTED_ROWS = 1u;   // k_bucket_scatter also copies token rows + meta into sorted order (coalesced reads in k_match_fast)
 constexpr u32 MAX_BUCKET_BITS = 18;   // locality buckets: 2^bits, bits = site_bits + sub_bits (engine.cu)
 constexpr u32 TOK8 = 8;              // levels kept in the per-topic 32-byte token row

@@ -130,6 +130,16 @@ struct GatherTarget { const GatherLayout* layout; char* const* blocks; u32 rank;
 // ---- the launch sequences ----------------------------------------------------------------------------------------------
 struct MatchScratch { u32 *tok, *tok8, *meta, *slow, *sort, *hist; Ctrl* ctrl; u64* gstack; Desc* gpool; };
 
+// What a match zeroes before it runs; nothing else of its scratch is cleared.  The whole control block, or all of it but
+// `cursor` when the call keeps the cursor (the chunks of one pipelined host call share one bump cursor over `out`; everything
+// else, item_cursor included, is per chunk), and the counts half of the locality histogram.
+struct ByteRange { void* p; size_t bytes; };
+struct MatchResets { ByteRange r[2]; };
+inline MatchResets match_resets(const MatchPlan& p, const MatchScratch& m, bool keep_cursor) {
+    const size_t skip = keep_cursor ? offsetof(Ctrl, item_cursor) : 0;
+    return MatchResets{{ByteRange{reinterpret_cast<char*>(m.ctrl) + skip, sizeof(Ctrl) - skip}, ByteRange{m.hist, p.nbuckets * sizeof(u32)}}};
+}
+
 // one batch: where its text comes from and where the results go
 struct MatchIO {
     const void* blob = nullptr; u64 blob_bytes = 0, readable_bytes = 0;   // readable: bytes the bulk tokeniser may read (at least blob_bytes)

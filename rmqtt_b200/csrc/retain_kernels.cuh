@@ -95,9 +95,12 @@ __device__ __forceinline__ void push_tasks(const RetainParams& p, RTask* out, u3
     if (nt == 0) return;
     const u32 sq = min(RQ - 1u, static_cast<u32>((static_cast<unsigned long long>(kb) * RQ) / max(p.v.n_kids, 1u)));
     const u32 at = atomicAdd(n_out + sq, nt);
-    if (at + nt > p.cap_items) { atomicOr(p.err, 1u); return; }
+    // on overflow the lookup is retried with a larger scratch, but the next round of THIS attempt still reads the slice up to
+    // cap_items: the tasks that fit are stored, so that it never reads an entry nobody wrote
+    const u32 fit = at < p.cap_items ? min(nt, p.cap_items - at) : 0u;
+    if (fit < nt) atomicOr(p.err, 1u);
     RTask* dst = out + static_cast<size_t>(sq) * p.cap_items + at;
-    for (u32 j = 0; j < nt; ++j) dst[j] = RTask{q, pos | (mode << 30), kb + j * RTASK_CHUNK, min(RTASK_CHUNK, kn - j * RTASK_CHUNK)};
+    for (u32 j = 0; j < fit; ++j) dst[j] = RTask{q, pos | (mode << 30), kb + j * RTASK_CHUNK, min(RTASK_CHUNK, kn - j * RTASK_CHUNK)};
 }
 
 // The record of the node a thread currently stands on.  `mask`: 32-bit Bloom mask over the tokens of its children (it

@@ -8,6 +8,10 @@
 #include <cuda_runtime.h>      // the emulation (this directory is first on the include path)
 
 #include <cstring>
+#include <memory>
+#ifdef EMU_ASAN
+#include <sanitizer/asan_interface.h>
+#endif
 #include <new>
 #include <vector>
 
@@ -21,18 +25,74 @@ namespace {
 
 constexpr u32 EMU_SMS = 2;               // the emulated part has two SMs: several CTAs per kernel, dynamic tile hand-out exercised
 
-// host memory standing in for cudaMalloc'd scratch: zeroed, 256-byte aligned, exactly the planned size (ASan sees its end)
+// Host memory standing in for cudaMalloc'd scratch, 256-byte aligned.  A fresh block holds POISON, not zeros:
+// a device allocation holds garbage, and the engine clears only what pipeline.cuh's match_resets names (retained lookups:
+// their control block and queue counters), so a read of scratch the call never wrote shows up as a wrong result.  GUARD bytes follow every block in the same allocation.  In the
+// plain build they hold POISON and intact() after the call catches a write past the block's end.  In the ASan build they
+// are also marked unaddressable, so ASan still reports any read or write past the block's end, as it would for an
+// allocation of exactly the block's size.
+constexpr u8 POISON = 0xA5;
+constexpr size_t GUARD = 256;
+#ifdef EMU_ASAN
+inline void guard_off(const void* p, size_t n) { ASAN_UNPOISON_MEMORY_REGION(p, n); }
+inline void guard_on(const void* p, size_t n) { ASAN_POISON_MEMORY_REGION(p, n); }
+#else
+inline void guard_off(const void*, size_t) {}
+inline void guard_on(const void*, size_t) {}
+#endif
+struct Block {
+    u8* p = nullptr;
+    size_t cap = 0;
+    Block() = default;
+    Block(const Block&) = delete;
+    Block& operator=(const Block&) = delete;
+    ~Block() { release(); }
+    void release() {
+        if (p) { guard_off(p + cap, GUARD); ::operator delete(p, std::align_val_t(256)); }
+        p = nullptr;
+    }
+    // exact: a block of exactly `bytes`; else the engine's DevBuf::ensure: grow (a fresh block) only when too small, keep the contents otherwise
+    template <class T> T* get(size_t bytes, bool exact = true, u8 fill = POISON) {
+        if (!p || (exact ? bytes != cap : bytes > cap)) {
+            const size_t ncap = exact || !p ? bytes : std::max(bytes, cap + cap / 2);
+            release();
+            cap = ncap;
+            p = static_cast<u8*>(::operator new(cap + GUARD, std::align_val_t(256)));
+            std::memset(p, fill, cap);
+            std::memset(p + cap, POISON, GUARD);
+            guard_on(p + cap, GUARD);
+        }
+        return reinterpret_cast<T*>(p);
+    }
+    bool intact() const {
+        if (!p) return true;
+        guard_off(p + cap, GUARD);
+        bool ok = true;
+        for (size_t i = 0; i < GUARD; ++i) ok &= p[cap + i] == POISON;
+        guard_on(p + cap, GUARD);
+        return ok;
+    }
+};
+// the retained lookup's scratch: poisoned as well (engine.cu clears its control block and queue counters, as the driver does)
 struct Arena {
-    std::vector<void*> blocks;
-    Arena() = default;
-    Arena(const Arena&) = delete;
-    Arena& operator=(const Arena&) = delete;
-    ~Arena() { for (void* p : blocks) ::operator delete(p, std::align_val_t(256)); }
-    template <class T> T* get(size_t bytes) {
-        void* p = ::operator new(std::max<size_t>(bytes, 1), std::align_val_t(256));
-        std::memset(p, 0, bytes);
-        blocks.push_back(p);
-        return static_cast<T*>(p);
+    std::vector<std::unique_ptr<Block>> blocks;
+    template <class T> T* get(size_t bytes) { blocks.emplace_back(new Block()); return blocks.back()->get<T>(bytes); }
+    bool intact() const { for (const auto& b : blocks) if (!b->intact()) return false; return true; }
+};
+
+// the scratch of one match context (engine.cu MatchCtx): fresh and exactly sized for every call, or kept across calls
+struct MatchBufs {
+    Block tok, tok8, meta, slow, sort, hist, ctrl, gstack, gpool;
+    MatchScratch get(const MatchPlan& p, bool exact) {
+        MatchScratch m{};
+        m.tok = tok.get<u32>(p.tok, exact); m.tok8 = tok8.get<u32>(p.tok8, exact); m.meta = meta.get<u32>(p.meta, exact); m.slow = slow.get<u32>(p.slow, exact);
+        m.sort = sort.get<u32>(p.sort, exact); m.hist = hist.get<u32>(p.hist, exact); m.ctrl = ctrl.get<Ctrl>(p.ctrl, exact); m.gstack = gstack.get<u64>(p.gstack, exact);
+        m.gpool = gpool.get<Desc>(p.gpool, exact);
+        return m;
+    }
+    bool intact() const {
+        for (const Block* b : {&tok, &tok8, &meta, &slow, &sort, &hist, &ctrl, &gstack, &gpool}) if (!b->intact()) return false;
+        return true;
     }
 };
 
@@ -137,17 +197,28 @@ struct EmuEngine {
     }
     RetainView rview() { return image ? dev_rview : retain_view(rtree, rtree.rkids.data(), rtree.redges.data(), rtree.rvals.data()); }
 
-    // one match through engine.cu's launch sequence, its scratch allocated by the plan; returns the control block
-    Ctrl match(const MatchIO& io, bool bulk) {
+    // scheduling knobs (gm_debug_knob) and the launch capacity of the small-graph form (0: the batch size + 37)
+    u32 tile_chunk = 1, diag_flags = 0, graph_cap = 0;
+    int k2_ctas = 0;
+    // keep_scratch: one scratch across calls, as a match context keeps it (grown only when too small); else a fresh one per call
+    bool keep_scratch = false;
+    MatchBufs kept;
+    bool overrun = false;                // a call wrote past the end of a scratch block (its guard bytes changed)
+
+    // one match through engine.cu's launch sequence, its scratch allocated by the plan and cleared as the engine clears it;
+    // returns the control block
+    Ctrl match(const MatchIO& io, bool bulk, bool keep_cursor = false) {
         const TrieView tv = view();
         MatchKnobs kn;
         kn.tok_bulk = bulk; kn.site_bits = site_bits; kn.pool_rows = pool_rows;
+        kn.tile_chunk = tile_chunk; kn.k2_ctas = k2_ctas; kn.diag_flags = diag_flags;
         const MatchPlan p = plan_match(static_cast<u32>(io.n), tv.max_depth, kn, EMU_SMS, io.hdr != nullptr);
-        Arena a;
-        MatchScratch m{};
-        m.tok = a.get<u32>(p.tok); m.tok8 = a.get<u32>(p.tok8); m.meta = a.get<u32>(p.meta); m.slow = a.get<u32>(p.slow); m.sort = a.get<u32>(p.sort);
-        m.hist = a.get<u32>(p.hist); m.ctrl = a.get<Ctrl>(p.ctrl); m.gstack = a.get<u64>(p.gstack); m.gpool = a.get<Desc>(p.gpool);
+        MatchBufs fresh;
+        MatchBufs& b = keep_scratch ? kept : fresh;
+        const MatchScratch m = b.get(p, !keep_scratch);
+        for (const ByteRange& r : match_resets(p, m, keep_cursor).r) std::memset(r.p, 0, r.bytes);
         launch_match(p, m, io, kn, tv, nullptr);
+        if (!b.intact()) overrun = true;
         return *m.ctrl;
     }
 };
@@ -208,17 +279,20 @@ uint64_t emu_retain_bulk_load(void* h, const char* blob, const uint32_t* offs, c
 //        bit 3 the batch is a SELECTION: row t matches entry sel[t] of the packed batch (n rows, n_entries entries; gm_match_args.d_sel),
 //        bit 4 the small-batch-graph form: the kernels are launched for a CAPACITY larger than the batch and read the real
 //              batch size / text length from a header in memory (engine.cu small_graph_match).
+//        bit 5 (with bit 0) raw descriptors: out_ids receives cap_ids descriptors (ref, cnt) as the kernels wrote them, unexpanded.
+// -60: a kernel wrote past the end of a scratch block.
 int32_t emu_match_ex(void* h, const char* blob_in, const uint32_t* offs, uint64_t n_entries, const uint32_t* sel, uint64_t n64, const uint32_t* trees, uint32_t flags,
                      gm_span* out_spans, uint32_t* out_ids, uint64_t cap_ids, uint64_t* needed, int32_t* status, uint64_t* work, uint32_t* deferred) {
     EmuEngine& e = *static_cast<EmuEngine*>(h);
-    const bool desc = flags & 1u, graph_form = flags & 16u;
+    const bool desc = flags & 1u, graph_form = flags & 16u, raw_desc = desc && (flags & 32u);
     if (!(flags & 8u)) sel = nullptr;
     const u32 n_real = static_cast<u32>(n64);
     *needed = 0;
     if (n_real == 0) return 0;
     if (!e.prepare(false)) return -7;
     const Text text(blob_in, offs[n_entries]);
-    const u32 n = graph_form ? n_real + 37u : n_real;            // launch size (rows beyond the real batch must stay untouched)
+    if (graph_form && e.graph_cap && e.graph_cap < n_real) return -2;
+    const u32 n = graph_form ? (e.graph_cap ? e.graph_cap : n_real + 37u) : n_real;   // launch size (rows beyond the real batch must stay untouched)
     const u32 hdr[4] = {n_real, text.bytes, 0u, 0u};
     std::vector<u32> offs_cap;
     if (graph_form) {                                             // the in-block holds capacity + 1 offsets; the tail is never read
@@ -227,7 +301,7 @@ int32_t emu_match_ex(void* h, const char* blob_in, const uint32_t* offs, uint64_
         offs = offs_cap.data();
     }
     std::vector<uint2> descs;
-    if (desc) descs.resize(cap_ids + 1);
+    if (desc && !raw_desc) descs.resize(cap_ids + 1);
     std::vector<int32_t> status_cap;
     std::vector<gm_span> spans_cap;
     for (u32 i = 0; i < n_real; ++i) status[i] = 0x7F7F7F7F;   // every row must be written by the tokeniser
@@ -237,9 +311,11 @@ int32_t emu_match_ex(void* h, const char* blob_in, const uint32_t* offs, uint64_
     io.blob = text.p; io.blob_bytes = text.bytes; io.readable_bytes = text.readable; io.offs = offs; io.sel = sel; io.n = n; io.trees = trees;
     io.hdr = graph_form ? hdr : nullptr;
     io.spans = graph_form ? spans_cap.data() : out_spans; io.status = graph_form ? status_cap.data() : status;
-    io.out = desc ? static_cast<void*>(descs.data()) : out_ids; io.cap = cap_ids;
+    io.out = desc && !raw_desc ? static_cast<void*>(descs.data()) : out_ids; io.cap = cap_ids;
     io.stats = flags & 4u; io.desc = desc;
+    e.overrun = false;
     const Ctrl ctrl = e.match(io, flags & 2u);
+    if (e.overrun) return -60;
     if (graph_form) {
         for (u32 i = n_real; i < n; ++i) if (status_cap[i] != 0x7F7F7F7F) return -50;      // a row beyond the real batch was touched
         for (u32 i = n_real; i < n; ++i) if (spans_cap[i].off != 0xABABABABu) return -51;
@@ -250,7 +326,7 @@ int32_t emu_match_ex(void* h, const char* blob_in, const uint32_t* offs, uint64_
     if (work) for (int k = 0; k < 4; ++k) work[k] = ctrl.stats[k];
     *needed = ctrl.cursor;
     if (ctrl.cursor > cap_ids) return -3;
-    if (!desc) return 0;
+    if (!desc || raw_desc) return 0;
     // descriptor mode: expand (ref, cnt) into ids out of the host mirror, per topic, so that the caller compares id lists
     std::vector<u32> ids_tmp;
     u64 w = 0;
@@ -278,6 +354,46 @@ int32_t emu_match_ex(void* h, const char* blob_in, const uint32_t* offs, uint64_
 int32_t emu_match(void* h, const char* blob_in, const uint32_t* offs, uint64_t n64, const uint32_t* trees, uint32_t flags, gm_span* out_spans, uint32_t* out_ids,
                   uint64_t cap_ids, uint64_t* needed, int32_t* status, uint64_t* work, uint32_t* deferred) {
     return emu_match_ex(h, blob_in, offs, n64, nullptr, n64, trees, flags & ~8u, out_spans, out_ids, cap_ids, needed, status, work, deferred);
+}
+
+// The pipelined host call (engine.cu match_host_impl): chunks of `chunk` rows, one after the other on ONE kept scratch; the
+// first chunk clears the whole control block, every later one all of it but the bump cursor over out_ids (keep_cursor).
+// flags: bit 1 the bulk-staged tokeniser.  Returns 0, -3 (*needed: ids needed) or -60 as emu_match_ex.
+int32_t emu_match_chunked(void* h, const char* blob_in, const uint32_t* offs, uint64_t n64, uint32_t flags, uint64_t chunk, gm_span* out_spans, uint32_t* out_ids,
+                          uint64_t cap_ids, uint64_t* needed, int32_t* status) {
+    EmuEngine& e = *static_cast<EmuEngine*>(h);
+    *needed = 0;
+    if (n64 == 0) return 0;
+    if (chunk == 0) return -2;
+    if (!e.prepare(false)) return -7;
+    const Text text(blob_in, offs[n64]);
+    for (u64 i = 0; i < n64; ++i) status[i] = 0x7F7F7F7F;
+    const bool keep = e.keep_scratch;
+    e.keep_scratch = true;
+    e.overrun = false;
+    unsigned long long cursor = 0;
+    for (u64 c0 = 0; c0 < n64; c0 += chunk) {
+        const u64 c1 = std::min<u64>(n64, c0 + chunk);
+        MatchIO io;
+        io.blob = text.p; io.blob_bytes = offs[c1]; io.readable_bytes = (offs[c1] + 15u) & ~15u; io.offs = offs + c0; io.n = c1 - c0;
+        io.spans = out_spans + c0; io.status = status + c0; io.out = out_ids; io.cap = cap_ids;
+        cursor = e.match(io, flags & 2u, c0 != 0).cursor;
+    }
+    e.keep_scratch = keep;
+    if (e.overrun) return -60;
+    *needed = cursor;
+    return cursor > cap_ids ? -3 : 0;
+}
+
+void emu_set_knobs(void* h, uint32_t tile_chunk, int32_t k2_ctas, uint32_t diag_flags, uint32_t graph_cap) {
+    EmuEngine& e = *static_cast<EmuEngine*>(h);
+    e.tile_chunk = tile_chunk; e.k2_ctas = k2_ctas; e.diag_flags = diag_flags; e.graph_cap = graph_cap;
+}
+// on != 0: one scratch kept across calls (a match context's); 0: a fresh, exactly sized one per call (the kept one is freed)
+void emu_keep_scratch(void* h, uint32_t on) {
+    EmuEngine& e = *static_cast<EmuEngine*>(h);
+    e.keep_scratch = on != 0;
+    if (!on) for (Block* b : {&e.kept.tok, &e.kept.tok8, &e.kept.meta, &e.kept.slow, &e.kept.sort, &e.kept.hist, &e.kept.ctrl, &e.kept.gstack, &e.kept.gpool}) { b->release(); b->cap = 0; }
 }
 
 // gm_partition_batch_device: k_partition.  counts[n_shards + 1] (the last entry = rows appended to sel)
@@ -329,7 +445,9 @@ int32_t emu_match_gather(void* gw, uint32_t rank, void* h, const char* blob_in, 
         MatchIO io;
         io.blob = text.p; io.blob_bytes = text.bytes; io.readable_bytes = text.readable; io.offs = offs; io.sel = sel; io.n = n;
         io.cap = G.slab_ids; io.status = status; io.gather = &target;
+        e.overrun = false;
         G.cursor[rank] = e.match(io, false).cursor;
+        if (e.overrun) return -60;
         if (G.cursor[rank] > G.slab_ids) return -3;
     }
     if (!direct && G.world > 1)
@@ -378,8 +496,10 @@ int32_t emu_retain_match(void* h, const char* blob_in, const uint32_t* offs, uin
     RetainScratch r{};
     r.tok = a.get<u32>(p.tok); r.tok8 = a.get<u32>(p.tok8); r.meta = a.get<u32>(p.meta); r.rq = a.get<u32>(p.rq); r.ctl = a.get<RCtl>(p.ctl);
     r.front[0] = a.get<RTask>(p.front); r.front[1] = a.get<RTask>(p.front); r.descs = a.get<RDesc>(p.descs);
+    std::memset(r.ctl, 0, p.ctl); std::memset(r.rq, 0, p.rq);        // what engine.cu clears before a retained lookup
     for (u32 i = 0; i < nq; ++i) status[i] = 0x7F7F7F7F;
     launch_retain(p, r, tv, rv, text.p, text.bytes, offs, out_spans, out_ids, cap_ids, status, stats_on != 0, nullptr);
+    if (!a.intact()) return -60;
     RCtl& ctl = *r.ctl;
     if (work) { work[0] = ctl.stats[0]; work[1] = ctl.stats[1]; }
     if (ctl.err) return -100 - static_cast<int32_t>(ctl.err);      // scratch overflow: bit 0 tasks, bit 1 descriptors (the engine grows and retries)
