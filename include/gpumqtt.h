@@ -307,6 +307,16 @@ void gm_batcher_destroy(gm_batcher* b);
 typedef struct gm_latency { double p50_us, p99_us, mean_us, max_us, topics_per_s, ids_per_topic; uint64_t samples; } gm_latency;
 int32_t gm_batcher_probe(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, uint32_t burst, uint32_t rounds,
                          uint32_t max_wait_us, gm_latency* out);
+/* The SUBSCRIBE side: RetainStorage::get is called once per subscription from many session tasks (rmqtt/src/session.rs:1336-1357).
+ * A retained batcher is the same gm_batcher over gm_retain_match_batch: gm_submit takes one topic FILTER, the callback receives
+ * the handles of the retained messages it matches (as gm_retain_match_batch returns them); status GM_ERR_INVALID_TOPIC for an
+ * invalid filter, or the batch's error for every filter of a failed batch.  gm_batcher_drain / gm_batcher_destroy work
+ * unchanged (destroy drains first); gm_submit_publish returns GM_ERR_INVALID_ARG (a PUBLISH topic is not a filter).  Lookups
+ * stay one at a time per engine; batches of up to 2048 filters run as one CUDA-graph launch.                                 */
+int32_t gm_retain_batcher_create(gm_engine* e, const gm_batcher_config* cfg, gm_batcher** out);
+/* gm_batcher_probe over a retained batcher: `blob` / `offsets` hold filters; ids_per_topic = retained handles per filter       */
+int32_t gm_retain_batcher_probe(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, uint32_t burst, uint32_t rounds,
+                                uint32_t max_wait_us, gm_latency* out);
 
 /* Churn probe: remove + re-add the given (filter, value) pairs cyclically from the calling thread at `target_ops_per_s`
  * (0 = unthrottled) for `duration_ms`, with a gm_flush every `flush_period_us` (0 = leave it to the matches' auto-flush).

@@ -100,6 +100,8 @@ extern "C" {
     pub fn gm_submit_publish(b: *mut gm_batcher, packet: *const u8, len: u32, cookie: u64) -> i32;
     pub fn gm_batcher_drain(b: *mut gm_batcher) -> i32;
     pub fn gm_batcher_destroy(b: *mut gm_batcher);
+    /// A batcher over gm_retain_match_batch: gm_submit takes one SUBSCRIBE filter, the callback gets its retained handles.
+    pub fn gm_retain_batcher_create(e: *mut gm_engine, cfg: *const gm_batcher_config, out: *mut *mut gm_batcher) -> i32;
     pub fn gm_sub_add_tree(e: *mut gm_engine, tree: u32, filter: *const u8, len: u32, value: u32, changed: *mut i32) -> i32;
     pub fn gm_sub_remove_tree(e: *mut gm_engine, tree: u32, filter: *const u8, len: u32, value: u32, changed: *mut i32) -> i32;
     pub fn gm_match_batch_trees(e: *mut gm_engine, topics_blob: *const u8, topic_offsets: *const u32, trees: *const u32, n: u64,
@@ -308,6 +310,8 @@ extern "C" {
     pub fn gm_publish_topic(packet: *const u8, len: u32, topic: *mut *const c_char, topic_len: *mut u32) -> i32;
     pub fn gm_batcher_probe(e: *mut gm_engine, blob: *const u8, offsets: *const u32, n: u64, burst: u32, rounds: u32, max_wait_us: u32,
                             out: *mut gm_latency) -> i32;
+    pub fn gm_retain_batcher_probe(e: *mut gm_engine, blob: *const u8, offsets: *const u32, n: u64, burst: u32, rounds: u32, max_wait_us: u32,
+                                   out: *mut gm_latency) -> i32;
     pub fn gm_churn_probe(e: *mut gm_engine, blob: *const u8, offsets: *const u32, values: *const u32, n: u64, target_ops_per_s: f64,
                           duration_ms: u32, flush_period_us: u32, out: *mut gm_churn) -> i32;
     // multi-GPU: communicator, device partition, the collective (NCCL form and the peer-memory form fused into the match kernels)

@@ -164,12 +164,20 @@ mod engine {
 
     impl Batcher {
         pub fn new(engine: std::sync::Arc<Engine>, max_batch: u32, max_wait_us: u32, dispatchers: u32) -> anyhow::Result<Self> {
+            Self::create(engine, max_batch, max_wait_us, dispatchers, false)
+        }
+        /// The retained batcher (`gm_retain_batcher_create`): one `submit` per SUBSCRIBE filter, the reply holds the handles of
+        /// the retained messages it matches.
+        pub fn retained(engine: std::sync::Arc<Engine>, max_batch: u32, max_wait_us: u32, dispatchers: u32) -> anyhow::Result<Self> {
+            Self::create(engine, max_batch, max_wait_us, dispatchers, true)
+        }
+        fn create(engine: std::sync::Arc<Engine>, max_batch: u32, max_wait_us: u32, dispatchers: u32, retained: bool) -> anyhow::Result<Self> {
             let cfg = sys::gm_batcher_config {
                 struct_size: std::mem::size_of::<sys::gm_batcher_config>() as u32, max_batch, max_wait_us, dispatchers, on_match, user: std::ptr::null_mut(),
             };
             let mut raw = std::ptr::null_mut();
-            let rc = unsafe { sys::gm_batcher_create(engine.0, &cfg, &mut raw) };
-            if rc != sys::GM_OK { return Err(engine.err("gm_batcher_create", rc)) }
+            let rc = unsafe { if retained { sys::gm_retain_batcher_create(engine.0, &cfg, &mut raw) } else { sys::gm_batcher_create(engine.0, &cfg, &mut raw) } };
+            if rc != sys::GM_OK { return Err(engine.err(if retained { "gm_retain_batcher_create" } else { "gm_batcher_create" }, rc)) }
             Ok(Self { raw, _engine: engine })
         }
         /// Never waits for the device; the reply arrives on the returned channel.
@@ -232,7 +240,7 @@ impl GpuRouterPlugin {
         log::info!("{name} GpuRouterPlugin cfg: {cfg:?}");
         let engine = Arc::new(Engine::new(cfg.device, cfg.filters_hint)?);
         let router = GpuRouter::new(scx.clone(), engine.clone(), &cfg)?;
-        let retainer = cfg.retain.then(|| GpuRetainer::new(engine.clone()));
+        let retainer = if cfg.retain { Some(GpuRetainer::new(engine.clone())?) } else { None };
         Ok(Self { scx, cfg, engine, router, retainer })
     }
 }
@@ -404,12 +412,17 @@ struct Slot { topic: TopicName, retain: Retain, expiry: Option<Instant> }
 #[derive(Clone)]
 pub struct GpuRetainer {
     engine: Arc<Engine>,
+    batcher: Arc<Batcher>,
     slots: Arc<DashMap<u32, Slot>>,
     next: Arc<AtomicU32>,
 }
 
 impl GpuRetainer {
-    fn new(engine: Arc<Engine>) -> Self { Self { engine, slots: Arc::new(DashMap::default()), next: Arc::new(AtomicU32::new(0)) } }
+    /// A reconnect storm resubscribes many sessions at once: their lookups share device batches instead of queueing one by one.
+    fn new(engine: Arc<Engine>) -> Result<Self> {
+        let batcher = Arc::new(Batcher::retained(engine.clone(), 2048, 100, 2)?);
+        Ok(Self { engine, batcher, slots: Arc::new(DashMap::default()), next: Arc::new(AtomicU32::new(0)) })
+    }
 
     /// retain.rs:118-128 (`remove_expired_messages`): the host decides what expired, the tree forgets it in one call
     async fn remove_expired_messages(&self) -> usize {
@@ -441,9 +454,7 @@ impl RetainStorage for GpuRetainer {
 
     /// retain.rs:152-169: expired entries are dropped, the rest cloned out
     async fn get(&self, topic_filter: &TopicFilter) -> Result<Vec<(TopicName, Retain)>> {
-        let (engine, filter) = (self.engine.clone(), topic_filter.to_string());
-        let mut replies = tokio::task::spawn_blocking(move || engine.retain_match(&[filter.as_str()])).await??;
-        let ids = replies.pop().unwrap_or(Ok(Vec::new())).map_err(|st| anyhow::anyhow!("invalid topic filter ({st})"))?;
+        let ids = self.batcher.submit(topic_filter.as_ref())?.await?.map_err(|st| anyhow::anyhow!("retained lookup failed ({st})"))?;
         let now = Instant::now();
         Ok(ids.into_iter().filter_map(|h| self.slots.get(&h).filter(|s| s.expiry.map(|t| t > now).unwrap_or(true)).map(|s| (s.topic.clone(), s.retain.clone()))).collect())
     }

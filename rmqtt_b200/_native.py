@@ -140,6 +140,8 @@ SIGNATURES = {
     "gm_batcher_drain": (_i32, [_vp]),
     "gm_batcher_destroy": (None, [_vp]),
     "gm_batcher_probe": (_i32, [_vp, _vp, _vp, _u64, _u32, _u32, _u32, _P(GmLatency)]),
+    "gm_retain_batcher_create": (_i32, [_vp, _P(GmBatcherConfig), _P(_vp)]),
+    "gm_retain_batcher_probe": (_i32, [_vp, _vp, _vp, _u64, _u32, _u32, _u32, _P(GmLatency)]),
     "gm_churn_probe": (_i32, [_vp, _vp, _vp, _vp, _u64, C.c_double, _u32, _u32, _P(GmChurn)]),
     "gm_relations_expand_device": (_i32, [_vp, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _vp]),
     "gm_relations_choose_device": (_i32, [_vp, _vp, _vp, _u64, _vp, _vp, _u64, _P(GmRelGroups), _vp, _vp]),

@@ -7,7 +7,8 @@
 // has waited `max_wait_us`.  With two (or more) dispatchers one batch is being collected while another is on the
 // device; the engine keeps several batches in flight (match contexts, engine.cu) and serves small ones as a single
 // CUDA-graph launch.  Results come back through a callback per topic (a Rust caller completes a oneshot / writes an
-// eventfd there).  Only the public C ABI is used here.
+// eventfd there).  Only the public C ABI is used here.  The same queue serves the retained lookup (retain_batcher.cpp): a
+// batcher holds the engine call it dispatches to (batcher_internal.h).
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -19,7 +20,7 @@
 #include <thread>
 #include <vector>
 
-#include "../../include/gpumqtt.h"
+#include "batcher_internal.h"
 
 namespace {
 using Clock = std::chrono::steady_clock;
@@ -36,6 +37,7 @@ struct Pending {
 
 struct gm_batcher {
     gm_engine* e = nullptr;
+    gm::BatcherTarget target{};
     gm_batcher_config cfg{};
     std::mutex mu;
     std::condition_variable cv_work, cv_drain;
@@ -81,12 +83,12 @@ struct gm_batcher {
             uint64_t needed = 0;
             int32_t rc;
             for (;;) {
-                rc = gm_match_batch(e, local.blob.data(), local.offs.data(), n, spans.data(), ids, ids_cap, &needed, status.data());
+                rc = target.call(e, local.blob.data(), local.offs.data(), n, spans.data(), ids, ids_cap, &needed, status.data());
                 if (rc != GM_ERR_CAPACITY || !grow_ids(needed)) break;
             }
             if (rc != GM_OK) {                      // the whole batch failed: every topic gets the error; say why (first few times)
                 static std::atomic<int> shown{0};
-                if (shown.fetch_add(1) < 5) fprintf(stderr, "libgpumqtt batcher: gm_match_batch(%llu topics) failed with %d: %s\n", (unsigned long long)n, rc, gm_last_error(e));
+                if (shown.fetch_add(1) < 5) fprintf(stderr, "libgpumqtt batcher: %s(%llu topics) failed with %d: %s\n", target.name, (unsigned long long)n, rc, gm_last_error(e));
             }
             for (uint64_t i = 0; i < n; ++i) {
                 const int32_t st = rc == GM_OK ? status[i] : rc;
@@ -102,12 +104,15 @@ struct gm_batcher {
     }
 };
 
-extern "C" {
+namespace {
+const gm::BatcherTarget kPublish{gm_match_batch, "gm_match_batch", true};
+}
 
-int32_t gm_batcher_create(gm_engine* e, const gm_batcher_config* cfg, gm_batcher** out) {
+int32_t gm::batcher_create(gm_engine* e, const gm_batcher_config* cfg, const BatcherTarget& target, gm_batcher** out) {
     if (!e || !cfg || !out || !cfg->on_match) return GM_ERR_INVALID_ARG;
     gm_batcher* b = new gm_batcher();
     b->e = e;
+    b->target = target;
     std::memcpy(&b->cfg, cfg, std::min<size_t>(cfg->struct_size ? cfg->struct_size : sizeof(gm_batcher_config), sizeof(gm_batcher_config)));
     if (b->cfg.max_batch == 0) b->cfg.max_batch = 4096;
     if (b->cfg.dispatchers == 0) b->cfg.dispatchers = 2;
@@ -116,6 +121,10 @@ int32_t gm_batcher_create(gm_engine* e, const gm_batcher_config* cfg, gm_batcher
     *out = b;
     return GM_OK;
 }
+
+extern "C" {
+
+int32_t gm_batcher_create(gm_engine* e, const gm_batcher_config* cfg, gm_batcher** out) { return gm::batcher_create(e, cfg, kPublish, out); }
 
 int32_t gm_submit(gm_batcher* b, const char* topic, uint32_t len, uint64_t cookie) {
     if (!b || (!topic && len)) return GM_ERR_INVALID_ARG;
@@ -161,6 +170,7 @@ int32_t gm_publish_topic(const uint8_t* packet, uint32_t len, const char** topic
 }
 
 int32_t gm_submit_publish(gm_batcher* b, const uint8_t* packet, uint32_t len, uint64_t cookie) {
+    if (b && !b->target.raw_packets) return GM_ERR_INVALID_ARG;        // a retained batcher takes filters, not PUBLISH topics
     const char* t = nullptr;
     uint32_t tl = 0;
     const int32_t rc = gm_publish_topic(packet, len, &t, &tl);
@@ -184,6 +194,8 @@ void gm_batcher_destroy(gm_batcher* b) {
     delete b;
 }
 
+}  // extern "C"
+
 // ---- closed-loop latency probe ------------------------------------------------------------------------------------
 namespace {
 struct Probe {
@@ -200,8 +212,8 @@ void probe_cb(void* user, uint64_t cookie, int32_t, const uint32_t*, uint32_t n_
 }
 }  // namespace
 
-int32_t gm_batcher_probe(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, uint32_t burst, uint32_t rounds, uint32_t max_wait_us,
-                         gm_latency* out) {
+int32_t gm::batcher_probe(gm_engine* e, const BatcherTarget& target, const char* blob, const uint32_t* offsets, uint64_t n, uint32_t burst, uint32_t rounds,
+                          uint32_t max_wait_us, gm_latency* out) {
     if (!e || !blob || !offsets || !out || n == 0 || burst == 0 || rounds == 0) return GM_ERR_INVALID_ARG;
     Probe p;
     const uint64_t total = static_cast<uint64_t>(burst) * rounds;
@@ -210,7 +222,7 @@ int32_t gm_batcher_probe(gm_engine* e, const char* blob, const uint32_t* offsets
     gm_batcher_config cfg{};
     cfg.struct_size = sizeof(cfg); cfg.max_batch = burst; cfg.max_wait_us = max_wait_us; cfg.dispatchers = 2; cfg.on_match = probe_cb; cfg.user = &p;
     gm_batcher* b = nullptr;
-    int32_t rc = gm_batcher_create(e, &cfg, &b);
+    int32_t rc = gm::batcher_create(e, &cfg, target, &b);
     if (rc != GM_OK) return rc;
     // warm-up round (graph capture, scratch allocation) — not measured
     {
@@ -245,6 +257,13 @@ int32_t gm_batcher_probe(gm_engine* e, const char* blob, const uint32_t* offsets
     out->topics_per_s = total / secs;
     out->ids_per_topic = static_cast<double>(p.ids.load()) / total;
     return GM_OK;
+}
+
+extern "C" {
+
+int32_t gm_batcher_probe(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, uint32_t burst, uint32_t rounds, uint32_t max_wait_us,
+                         gm_latency* out) {
+    return gm::batcher_probe(e, kPublish, blob, offsets, n, burst, rounds, max_wait_us, out);
 }
 
 // ---- churn probe: subscribe / unsubscribe load against a running engine --------------------------------------------

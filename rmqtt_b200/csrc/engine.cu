@@ -148,6 +148,7 @@ struct gm_engine {
     DevBuf d_rnodes, d_rkids, d_redges, d_rvals;
     DevBuf d_rfront[2], d_rdescs, d_rctl, d_rq, d_rstage[5];
     u32 r_cap_items = 1u << 22, r_cap_desc = 1u << 22;   // totals over the RQ slices of each queue
+    struct SmallGraph* rsmall[2] = {nullptr, nullptr};   // small retained lookups as one CUDA-graph launch (small_graph_retain; mu_ret)
     u64 launches = 0;
     // fused gather over peer memory (comm.cuh): one block per rank holding every rank's slab; the peers' blocks are opened by CUDA IPC
     struct Gather : GatherLayout {
@@ -443,10 +444,10 @@ struct gm_engine {
     }
 
     // ---- retained lookup (pipeline.cuh): tokenise filters -> frontier BFS (one step kernel per tree level) -> publish ----
-    int enqueue_retain(const void* d_blob_, u64 blob_bytes, const u32* d_offs_, u64 n, gm_span* d_spans_, u32* d_ids_, u64 cap_ids, int32_t* d_status_, cudaStream_t s) {
-        std::lock_guard<std::mutex> gd(mu_dev);     // enqueue only; the caller (holding mu_ret) synchronises afterwards without it
+    // The scratch of a lookup of `n` filters (caller holds mu_dev).  Retained lookups use devctx's token scratch and the
+    // engine's queues; their pointers and the slice capacities are what a captured retained graph bakes in (retain_sig).
+    int retain_scratch(const RetainPlan& p, RetainScratch& r) {
         MatchCtx& c = devctx;
-        const RetainPlan p = plan_retain(static_cast<u32>(n), dev_rview.max_depth, r_cap_items, r_cap_desc, num_sms);
         CUDA_TRY(c.d_tok.ensure(p.tok));
         CUDA_TRY(c.d_tok8.ensure(p.tok8));
         CUDA_TRY(c.d_meta.ensure(p.meta));
@@ -455,23 +456,46 @@ struct gm_engine {
         CUDA_TRY(d_rfront[0].ensure(p.front));
         CUDA_TRY(d_rfront[1].ensure(p.front));
         CUDA_TRY(d_rdescs.ensure(p.descs));
-        CUDA_TRY(cudaStreamWaitEvent(s, ev_flush, 0));
-        if (c.recorded) CUDA_TRY(cudaStreamWaitEvent(s, c.ev_done, 0));
-        CUDA_TRY(cudaMemsetAsync(d_rctl.p, 0, p.ctl, s));
-        CUDA_TRY(cudaMemsetAsync(d_rq.p, 0, p.rq, s));
-        RetainScratch r{};
+        r = RetainScratch{};
         r.tok = c.d_tok.as<u32>(); r.tok8 = c.d_tok8.as<u32>(); r.meta = c.d_meta.as<u32>(); r.rq = d_rq.as<u32>(); r.ctl = d_rctl.as<RCtl>();
         r.front[0] = d_rfront[0].as<RTask>(); r.front[1] = d_rfront[1].as<RTask>(); r.descs = d_rdescs.as<RDesc>();
+        return GM_OK;
+    }
+    u64 retain_sig() const {
+        u64 h = 0x9E3779B97F4A7C15ull;
+        for (const DevBuf* b : {&devctx.d_tok, &devctx.d_tok8, &devctx.d_meta, &d_rq, &d_rctl, &d_rfront[0], &d_rfront[1], &d_rdescs}) h = (h ^ reinterpret_cast<uintptr_t>(b->p)) * 0x100000001B3ull;
+        return (h ^ r_cap_items) * 0x100000001B3ull ^ r_cap_desc;
+    }
+    // `hdr` (small-graph form, small_graph_retain): n is the capacity and the caller holds mu_dev while it captures — no waits
+    // on other streams' events, no completion or timing events (the caller orders the graph launch itself)
+    int enqueue_retain(const void* d_blob_, u64 blob_bytes, const u32* d_offs_, u64 n, gm_span* d_spans_, u32* d_ids_, u64 cap_ids, int32_t* d_status_, cudaStream_t s,
+                       const u32* hdr = nullptr) {
+        std::unique_lock<std::mutex> gd(mu_dev, std::defer_lock);     // enqueue only; the caller (holding mu_ret) synchronises afterwards without it
+        if (!hdr) gd.lock();
+        MatchCtx& c = devctx;
+        const RetainPlan p = plan_retain(static_cast<u32>(n), dev_rview.max_depth, r_cap_items, r_cap_desc, num_sms);
+        RetainScratch r;
+        int st = retain_scratch(p, r);
+        if (st != GM_OK) return st;
+        if (!hdr) {
+            CUDA_TRY(cudaStreamWaitEvent(s, ev_flush, 0));
+            if (c.recorded) CUDA_TRY(cudaStreamWaitEvent(s, c.ev_done, 0));
+        }
+        CUDA_TRY(cudaMemsetAsync(d_rctl.p, 0, p.ctl, s));
+        CUDA_TRY(cudaMemsetAsync(d_rq.p, 0, p.rq, s));
+        const bool timing = hdr == nullptr;
         cudaEvent_t* ev_t = ev_ring[ring_n % RING];
         cudaError_t ev = cudaSuccess;
-        launch_retain(p, r, dev_view, dev_rview, d_blob_, blob_bytes, d_offs_, d_spans_, d_ids_, cap_ids, d_status_, knobs.retain_stats, s,
-                      [&](int k) { if (ev == cudaSuccess) ev = cudaEventRecord(ev_t[k], s); });
+        launch_retain(p, r, dev_view, dev_rview, d_blob_, blob_bytes, d_offs_, d_spans_, d_ids_, cap_ids, d_status_, knobs.retain_stats && !hdr, s, hdr,
+                      [&](int k) { if (timing && ev == cudaSuccess) ev = cudaEventRecord(ev_t[k], s); });
         CUDA_TRY(ev);
         CUDA_TRY(cudaGetLastError());
-        ring_n++;
-        launches += 4 + p.depth + 1;
-        CUDA_TRY(cudaEventRecord(c.ev_done, s));
-        c.recorded = true;
+        if (!hdr) {
+            ring_n++;
+            launches += 4 + p.depth + 1;
+            CUDA_TRY(cudaEventRecord(c.ev_done, s));
+            c.recorded = true;
+        }
         return GM_OK;
     }
 
@@ -573,6 +597,7 @@ void gm_destroy(gm_engine* e) {
     cudaDeviceSynchronize();
     e->free_retired(true);
     for (MatchCtx* cx : e->all_ctxs()) cx->destroy();
+    for (auto& g : e->rsmall) if (g) { small_graph_destroy(g); g = nullptr; }
     for (DevBuf* b : {&e->d_cfilter, &e->d_tree_slots, &e->d_edges, &e->d_ranges, &e->d_values, &e->d_dict, &e->d_pool, &e->d_patch, &e->d_rnodes, &e->d_rkids, &e->d_redges,
                       &e->d_rvals, &e->d_rfront[0], &e->d_rfront[1], &e->d_rdescs, &e->d_rctl, &e->d_rq, &e->d_rstage[0], &e->d_rstage[1], &e->d_rstage[2],
                       &e->d_rstage[3], &e->d_rstage[4]})
@@ -736,7 +761,8 @@ int32_t gm_match_batch_device_ex(gm_engine* e, const gm_match_args* a) {
 // is captured ONCE into a CUDA graph sized for the tier's capacity; the real batch size and text length travel in the
 // first words of the in-block (`hdr`), which the kernels read at run time.  A call then is: fill the pinned in-block,
 // cudaGraphLaunch, wait for one event, copy the results out of the pinned out-block.  The kernels carry the table view
-// by value, so the graph is re-captured (cudaGraphExecUpdate) when a flush has changed the view.
+// by value, so the graph is re-captured (cudaGraphExecUpdate) when a flush has changed the view.  Small retained lookups
+// (small_graph_retain) use the same tiers, blocks and capture helper.
 struct SmallGraph {
     u32 cap_n = 0, cap_blob = 0, cap_out = 0;
     size_t elem = 0;
@@ -755,27 +781,72 @@ static void small_graph_destroy(SmallGraph* g) {
     delete g;
 }
 
+// Capacity tiers: tier 0 holds up to 64 rows and 8 KiB of text, tier 1 up to 2048 rows and 192 KiB; their outputs hold
+// 4096 and 128 K elements (ids, or 8-byte descriptors).  -1: the batch is larger than both.
+static int small_graph_tier(u64 n, u64 blob_bytes) {
+    if (n <= 64 && blob_bytes <= 8 * 1024) return 0;
+    if (n <= 2048 && blob_bytes <= 192 * 1024) return 1;
+    return -1;
+}
+
+// in-block:  {n, text bytes} (16 B) | offsets [cap_n + 1] | trees [cap_n] | text (256-aligned)
+// out-block: head (32 B: the match's cursor, or the retained lookup's RCtl head) | spans [cap_n] | status [cap_n] | output (256-aligned)
+static int small_graph_new(SmallGraph*& g, int tier) {
+    g = new SmallGraph();
+    g->cap_n = tier == 0 ? 64u : 2048u; g->cap_blob = tier == 0 ? 8u * 1024u : 192u * 1024u; g->cap_out = tier == 0 ? 4096u : 128u * 1024u;
+    g->off_offs = 16; g->off_trees = g->off_offs + (g->cap_n + 1) * sizeof(u32); g->off_blob = (g->off_trees + g->cap_n * sizeof(u32) + 255) & ~size_t(255);
+    g->in_bytes = g->off_blob + g->cap_blob + 32;
+    g->off_spans = 32; g->off_status = g->off_spans + g->cap_n * sizeof(gm_span); g->off_out = (g->off_status + g->cap_n * sizeof(int32_t) + 255) & ~size_t(255);
+    g->out_bytes = g->off_out + static_cast<size_t>(g->cap_out) * 8;
+    CUDA_TRY(cudaMallocHost(&g->h_in, g->in_bytes));
+    CUDA_TRY(cudaMallocHost(&g->h_out, g->out_bytes));
+    CUDA_TRY(g->d_in.ensure(g->in_bytes));
+    CUDA_TRY(g->d_out.ensure(g->out_bytes));
+    std::memset(g->h_in, 0, g->in_bytes);
+    return GM_OK;
+}
+
+// Captures  H2D(in-block) -> enqueue(s) -> D2H(out-block)  on `s` unless the graph is current: captured for this view,
+// this scratch and this output element size.  An existing executable graph is updated in place (cudaGraphExecUpdate) and
+// re-instantiated only when the update is refused (the topology changed: another round count, another grid).
+template <class Enqueue>
+static int small_graph_refresh(SmallGraph* g, cudaStream_t s, u64 view_epoch, u64 scratch_sig, size_t elem, Enqueue&& enqueue) {
+    if (g->exec && g->view_epoch == view_epoch && g->elem == elem && g->scratch_sig == scratch_sig) return GM_OK;
+    cudaGraph_t graph = nullptr;
+    CUDA_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
+    cudaError_t ce = cudaMemcpyAsync(g->d_in.p, g->h_in, g->in_bytes, cudaMemcpyHostToDevice, s);
+    int st = ce == cudaSuccess ? enqueue(s) : GM_ERR_CUDA;
+    if (st == GM_OK) ce = cudaMemcpyAsync(g->h_out, g->d_out.p, g->out_bytes, cudaMemcpyDeviceToHost, s);
+    cudaError_t ee = cudaStreamEndCapture(s, &graph);
+    if (st != GM_OK || ce != cudaSuccess || ee != cudaSuccess) { if (graph) cudaGraphDestroy(graph); g_err = "small-batch graph capture failed"; return st != GM_OK ? st : GM_ERR_CUDA; }
+    bool ok = false;
+    if (g->exec) {
+        cudaGraphExecUpdateResultInfo info{};
+        ok = cudaGraphExecUpdate(g->exec, graph, &info) == cudaSuccess;
+        if (!ok) { cudaGetLastError(); cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
+    }
+    if (!ok) { const cudaError_t ie = cudaGraphInstantiate(&g->exec, graph, 0); if (ie != cudaSuccess) { cudaGraphDestroy(graph); g->exec = nullptr; CUDA_TRY(ie); } }
+    cudaGraphDestroy(graph);
+    g->view_epoch = view_epoch; g->elem = elem; g->scratch_sig = scratch_sig;
+    return GM_OK;
+}
+
+// fill the pinned in-block: {n, text bytes} | offsets re-based to 0 | text
+static void small_graph_fill(SmallGraph* g, const char* blob, const uint32_t* offsets, uint64_t n) {
+    const u64 b0 = offsets[0], blob_bytes = offsets[n] - b0;
+    u32* hdr = reinterpret_cast<u32*>(g->h_in);
+    hdr[0] = static_cast<u32>(n); hdr[1] = static_cast<u32>(blob_bytes);
+    u32* ho = reinterpret_cast<u32*>(g->h_in + g->off_offs);
+    for (u64 i = 0; i <= n; ++i) ho[i] = static_cast<u32>(offsets[i] - b0);
+    if (blob_bytes) std::memcpy(g->h_in + g->off_blob, blob + b0, blob_bytes);
+}
+
 static int small_graph_match(gm_engine* e, MatchCtx& c, std::unique_lock<std::mutex>& gd, const char* blob, const uint32_t* offsets, uint64_t n,
                              gm_span* out_spans, void* out, size_t elem, uint64_t cap_user, uint64_t* needed, int32_t* status, const uint32_t* trees) {
-    const u64 b0 = offsets[0], blob_bytes = offsets[n] - b0;
-    int tier;
-    if (n <= 64 && blob_bytes <= 8 * 1024) tier = 0;
-    else if (n <= 2048 && blob_bytes <= 192 * 1024) tier = 1;
-    else return GM_SMALL_NOT_APPLICABLE;
+    const int tier = small_graph_tier(n, offsets[n] - offsets[0]);
+    if (tier < 0) return GM_SMALL_NOT_APPLICABLE;
     SmallGraph*& g = c.small[tier];
-    if (!g) {
-        g = new SmallGraph();
-        g->cap_n = tier == 0 ? 64u : 2048u; g->cap_blob = tier == 0 ? 8u * 1024u : 192u * 1024u; g->cap_out = tier == 0 ? 4096u : 128u * 1024u;
-        g->off_offs = 16; g->off_trees = g->off_offs + (g->cap_n + 1) * sizeof(u32); g->off_blob = (g->off_trees + g->cap_n * sizeof(u32) + 255) & ~size_t(255);
-        g->in_bytes = g->off_blob + g->cap_blob + 32;
-        g->off_spans = 16; g->off_status = g->off_spans + g->cap_n * sizeof(gm_span); g->off_out = (g->off_status + g->cap_n * sizeof(int32_t) + 255) & ~size_t(255);
-        g->out_bytes = g->off_out + static_cast<size_t>(g->cap_out) * 8;
-        CUDA_TRY(cudaMallocHost(&g->h_in, g->in_bytes));
-        CUDA_TRY(cudaMallocHost(&g->h_out, g->out_bytes));
-        CUDA_TRY(g->d_in.ensure(g->in_bytes));
-        CUDA_TRY(g->d_out.ensure(g->out_bytes));
-        std::memset(g->h_in, 0, g->in_bytes);
-    }
+    if (!g) { int st = small_graph_new(g, tier); if (st != GM_OK) return st; }
     const bool desc = elem == 8;
     auto enqueue = [&](cudaStream_t s) -> int {
         char* di = static_cast<char*>(g->d_in.p);
@@ -800,30 +871,8 @@ static int small_graph_match(gm_engine* e, MatchCtx& c, std::unique_lock<std::mu
         if (st != GM_OK) return st;
         CUDA_TRY(cudaStreamSynchronize(c.sc));
     }
-    if (!g->exec || g->view_epoch != e->view_epoch || g->elem != elem || g->scratch_sig != c.scratch_sig()) {
-        cudaGraph_t graph = nullptr;
-        CUDA_TRY(cudaStreamBeginCapture(c.sc, cudaStreamCaptureModeRelaxed));
-        cudaError_t ce = cudaMemcpyAsync(g->d_in.p, g->h_in, g->in_bytes, cudaMemcpyHostToDevice, c.sc);
-        int st = ce == cudaSuccess ? enqueue(c.sc) : GM_ERR_CUDA;
-        if (st == GM_OK) ce = cudaMemcpyAsync(g->h_out, g->d_out.p, g->out_bytes, cudaMemcpyDeviceToHost, c.sc);
-        cudaError_t ee = cudaStreamEndCapture(c.sc, &graph);
-        if (st != GM_OK || ce != cudaSuccess || ee != cudaSuccess) { if (graph) cudaGraphDestroy(graph); g_err = "small-batch graph capture failed"; return st != GM_OK ? st : GM_ERR_CUDA; }
-        bool ok = false;
-        if (g->exec) {
-            cudaGraphExecUpdateResultInfo info{};
-            ok = cudaGraphExecUpdate(g->exec, graph, &info) == cudaSuccess;
-            if (!ok) { cudaGetLastError(); cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
-        }
-        if (!ok) CUDA_TRY(cudaGraphInstantiate(&g->exec, graph, 0));
-        cudaGraphDestroy(graph);
-        g->view_epoch = e->view_epoch; g->elem = elem; g->scratch_sig = c.scratch_sig();
-    }
-    // fill the pinned in-block: {n, text bytes} | offsets re-based to 0 | text
-    u32* hdr = reinterpret_cast<u32*>(g->h_in);
-    hdr[0] = static_cast<u32>(n); hdr[1] = static_cast<u32>(blob_bytes);
-    u32* ho = reinterpret_cast<u32*>(g->h_in + g->off_offs);
-    for (u64 i = 0; i <= n; ++i) ho[i] = static_cast<u32>(offsets[i] - b0);
-    if (blob_bytes) std::memcpy(g->h_in + g->off_blob, blob + b0, blob_bytes);
+    { int st = small_graph_refresh(g, c.sc, e->view_epoch, c.scratch_sig(), elem, enqueue); if (st != GM_OK) return st; }
+    small_graph_fill(g, blob, offsets, n);
     if (trees) std::memcpy(g->h_in + g->off_trees, trees, n * sizeof(u32)); else std::memset(g->h_in + g->off_trees, 0, n * sizeof(u32));
     CUDA_TRY(cudaStreamWaitEvent(c.sc, e->ev_flush, 0));
     CUDA_TRY(cudaGraphLaunch(g->exec, c.sc));
@@ -839,6 +888,70 @@ static int small_graph_match(gm_engine* e, MatchCtx& c, std::unique_lock<std::mu
     if (total > cap_user) { g_err = "output buffer too small"; return GM_ERR_CAPACITY; }
     std::memcpy(out_spans, g->h_out + g->off_spans, n * sizeof(gm_span));
     if (total) std::memcpy(out, g->h_out + g->off_out, total * elem);
+    return GM_OK;
+}
+
+// A retained lookup of 1 .. 2048 filters as ONE graph launch on devctx's stream (caller holds mu_ret):
+//     H2D(in-block) -> memsets of RCtl and the rq counters -> k_tokenize -> k_retain_init -> k_retain_round x (depth + 1)
+//     -> k_retain_scan -> k_retain_expand -> D2D of the RCtl head {grand, stats, err} into the out-block -> D2H(out-block)
+// The round count follows max_depth and RetainParams carries the root record and the slice capacities by value, so a flush
+// (view_epoch), a re-allocated scratch or new capacities (retain_sig) re-capture it.  GM_SMALL_NOT_APPLICABLE: too large for
+// a tier, a frontier or descriptor overflow, or more ids than the tier holds — the caller runs the pipelined lookup, which
+// grows the scratch and returns the same results.
+static int small_graph_retain(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, gm_span* out_spans, uint32_t* out_ids, uint64_t cap_ids,
+                              uint64_t* needed, int32_t* status) {
+    const int tier = small_graph_tier(n, offsets[n] - offsets[0]);
+    if (tier < 0) return GM_SMALL_NOT_APPLICABLE;
+    SmallGraph*& g = e->rsmall[tier];
+    if (!g) { int st = small_graph_new(g, tier); if (st != GM_OK) return st; }
+    MatchCtx& c = e->devctx;
+    std::unique_lock<std::mutex> gd(e->mu_dev);
+    auto enqueue = [&](cudaStream_t s) -> int {
+        char* di = static_cast<char*>(g->d_in.p);
+        char* dout = static_cast<char*>(g->d_out.p);
+        int st = e->enqueue_retain(di + g->off_blob, g->cap_blob, reinterpret_cast<const u32*>(di + g->off_offs), g->cap_n, reinterpret_cast<gm_span*>(dout + g->off_spans),
+                                   reinterpret_cast<u32*>(dout + g->off_out), g->cap_out, reinterpret_cast<int32_t*>(dout + g->off_status), s, reinterpret_cast<const u32*>(di));
+        if (st != GM_OK) return st;
+        static_assert(offsetof(RCtl, err) + sizeof(u32) <= 32, "the out-block head holds RCtl up to err");
+        CUDA_TRY(cudaMemcpyAsync(dout, e->d_rctl.p, 32, cudaMemcpyDeviceToDevice, s));
+        return GM_OK;
+    };
+    // devctx's scratch is shared with the device-buffer match entry points (other streams): order after them and the last flush
+    auto order = [&]() -> int {
+        CUDA_TRY(cudaStreamWaitEvent(c.sc, e->ev_flush, 0));
+        if (c.recorded) CUDA_TRY(cudaStreamWaitEvent(c.sc, c.ev_done, 0));
+        return GM_OK;
+    };
+    {   // size the scratch for the tier outside any capture (a graph must not allocate); the first time, also one empty (n = 0) pass
+        RetainScratch r;
+        int st = e->retain_scratch(plan_retain(g->cap_n, e->dev_rview.max_depth, e->r_cap_items, e->r_cap_desc, e->num_sms), r);
+        if (st == GM_OK && !g->warmed) {
+            if ((st = order()) != GM_OK) return st;
+            CUDA_TRY(cudaMemsetAsync(g->d_in.p, 0, g->in_bytes, c.sc));
+            if ((st = enqueue(c.sc)) != GM_OK) return st;
+            CUDA_TRY(cudaEventRecord(c.ev_done, c.sc));
+            CUDA_TRY(cudaStreamSynchronize(c.sc));
+            g->warmed = true;
+        }
+        if (st != GM_OK) return st;
+    }
+    { int st = small_graph_refresh(g, c.sc, e->view_epoch, e->retain_sig(), sizeof(u32), enqueue); if (st != GM_OK) return st; }
+    small_graph_fill(g, blob, offsets, n);
+    { int st = order(); if (st != GM_OK) return st; }
+    CUDA_TRY(cudaGraphLaunch(g->exec, c.sc));
+    CUDA_TRY(cudaEventRecord(c.ev_done, c.sc));
+    c.recorded = true;
+    e->launches += 4 + e->dev_rview.max_depth + 1;
+    gd.unlock();
+    CUDA_TRY(cudaStreamSynchronize(c.sc));
+    RCtl head;
+    std::memcpy(static_cast<void*>(&head), g->h_out, offsetof(RCtl, err) + sizeof(u32));
+    if (head.err != 0 || head.grand > g->cap_out) return GM_SMALL_NOT_APPLICABLE;
+    if (needed) *needed = head.grand;
+    std::memcpy(status, g->h_out + g->off_status, n * sizeof(int32_t));
+    std::memcpy(out_spans, g->h_out + g->off_spans, n * sizeof(gm_span));
+    if (head.grand > cap_ids) { g_err = "out_ids too small"; return GM_ERR_CAPACITY; }
+    if (head.grand) std::memcpy(out_ids, g->h_out + g->off_out, head.grand * sizeof(u32));
     return GM_OK;
 }
 
@@ -1054,6 +1167,10 @@ int32_t gm_retain_match_batch(gm_engine* e, const char* blob, const uint32_t* of
     CUDA_TRY(cudaSetDevice(e->device));
     std::lock_guard<std::mutex> gr(e->mu_ret);
     { int st = auto_flush(e, true); if (st != GM_OK) return st; }
+    if (e->knobs.small_graphs && !e->knobs.retain_stats) {      // (the per-round diagnostics come from the pipelined path)
+        int st = small_graph_retain(e, blob, offsets, n, out_spans, out_ids, cap_ids, needed, status);
+        if (st != GM_SMALL_NOT_APPLICABLE) return st;
+    }
     const u64 blob_bytes = offsets[n];
     MatchCtx& c = e->devctx;                          // staging of the retained host call (guarded by mu_ret)
     cudaStream_t s = c.sc;

@@ -213,20 +213,21 @@ inline void launch_match(const MatchPlan& p, const MatchScratch& m, const MatchI
 struct RetainScratch { u32 *tok, *tok8, *meta, *rq; RCtl* ctl; RTask* front[2]; RDesc* descs; };
 
 // k_tokenize -> k_retain_init -> k_retain_round x (depth + 1) -> k_retain_scan -> k_retain_expand.  `at(k)` runs before the
-// tokeniser (0), after it (1), after the last round (2) and after the expansion (3).
+// tokeniser (0), after it (1), after the last round (2) and after the expansion (3).  `hdr` (small-graph form, as MatchIO::hdr):
+// {n, blob_bytes} in memory, read at run time; p.nq is then the capacity.  Without it the launch is the pipelined lookup of nq filters.
 template <class Hook = NoHook>
 inline void launch_retain(const RetainPlan& p, const RetainScratch& r, const TrieView& tv, const RetainView& rv, const void* blob, u64 blob_bytes, const u32* offs,
-                          gm_span* spans, u32* ids, u64 cap_ids, int32_t* status, bool stats, cudaStream_t s, Hook at = {}) {
+                          gm_span* spans, u32* ids, u64 cap_ids, int32_t* status, bool stats, cudaStream_t s, const u32* hdr = nullptr, Hook at = {}) {
     const u32 nq = p.nq, depth = p.depth;
     u32* qtotal = r.rq;
     u32* qbase = qtotal + nq;
     u32* qcur = qbase + nq;
     at(0);
-    GM_LAUNCH(k_tokenize<false>, p.tok_grid, TOK_THREADS, 0, s, static_cast<const u8*>(blob), static_cast<u32>(blob_bytes), static_cast<u32>(blob_bytes), offs, nullptr, nq, nullptr, tv,
+    GM_LAUNCH(k_tokenize<false>, p.tok_grid, TOK_THREADS, 0, s, static_cast<const u8*>(blob), static_cast<u32>(blob_bytes), static_cast<u32>(blob_bytes), offs, nullptr, nq, hdr, tv,
               p.tok_levels, r.tok8, r.tok, r.meta, status, nullptr, nullptr, 0u, 0u);
     at(1);
     RetainParams rp{};
-    rp.v = rv; rp.qtok8 = r.tok8; rp.qtok = r.tok; rp.qmeta = r.meta; rp.nq = nq; rp.tok_levels = p.tok_levels;
+    rp.v = rv; rp.qtok8 = r.tok8; rp.qtok = r.tok; rp.qmeta = r.meta; rp.nq = nq; rp.n_ptr = hdr; rp.tok_levels = p.tok_levels;
     rp.descs = r.descs; rp.n_desc = r.ctl->n_desc; rp.cap_items = p.slice_items; rp.cap_desc = p.slice_desc;
     rp.qtotal = qtotal; rp.err = &r.ctl->err;
     rp.stats = r.ctl->stats;
@@ -239,7 +240,7 @@ inline void launch_retain(const RetainPlan& p, const RetainScratch& r, const Tri
     for (u32 lvl = 0; lvl <= depth; ++lvl)
         GM_LAUNCH(krr, p.round_grid, 256, 0, s, rp, r.front[lvl & 1], r.ctl->round_counts(lvl), r.front[(lvl + 1) & 1], r.ctl->round_counts(lvl + 1), r.ctl->claim(depth, lvl));
     at(2);
-    GM_LAUNCH(k_retain_scan, 1, 1024, 0, s, qtotal, nq, qbase, reinterpret_cast<uint2*>(spans), &r.ctl->grand);
+    GM_LAUNCH(k_retain_scan, 1, 1024, 0, s, qtotal, nq, hdr, qbase, reinterpret_cast<uint2*>(spans), &r.ctl->grand);
     GM_LAUNCH(k_retain_expand, p.expand_grid, 256, 0, s, r.descs, r.ctl->n_desc, p.slice_desc, rv.vals, qbase, qcur, ids, cap_ids);
     at(3);
 }

@@ -37,7 +37,8 @@ struct RetainParams {
     const u32* qtok8;    // [nq][8]  filter levels 0..7
     const u32* qtok;     // [tok_levels][nq]  levels >= 8
     const u32* qmeta;    // [nq]
-    u32 nq, tok_levels;
+    u32 nq, tok_levels;  // nq: rows of the launch (the row stride of qtok); with n_ptr a capacity
+    const u32* n_ptr;    // small-batch graphs: the real filter count lives in device memory (rows at or past it are not touched)
     RDesc* descs;
     u32* n_desc;         // [RQ]
     u32 cap_items, cap_desc;   // per SLICE
@@ -194,8 +195,9 @@ template <bool STATS>
 __global__ void __launch_bounds__(256)
 k_retain_init(RetainParams p, RTask* out, u32* n_out) {
     const u32 q = blockIdx.x * blockDim.x + threadIdx.x;
+    const u32 n_act = p.n_ptr ? min(p.nq, *p.n_ptr) : p.nq;
     unsigned long long visited = 0, probes = 0;
-    if (q < p.nq) {
+    if (q < n_act) {
         const u32 m = p.qmeta[q];
         if (!(m & META_INVALID))
             retain_chain<STATS>(p, out, n_out, (q >> 5) % RQ, q, m & META_NLEV_MASK, 0u,
@@ -311,10 +313,12 @@ k_retain_round(RetainParams p, const RTask* __restrict__ in, const u32* __restri
     }
 }
 
-// Exclusive scan of qtotal -> qbase, spans; single block (nq is a batch of SUBSCRIBE filters).
+// Exclusive scan of qtotal -> qbase, spans; single block (nq is a batch of SUBSCRIBE filters).  n_ptr (small-batch graphs):
+// the real filter count, read from device memory; nq is then the capacity.
 __global__ void __launch_bounds__(1024)
-k_retain_scan(const u32* __restrict__ qtotal, u32 nq, u32* __restrict__ qbase, uint2* __restrict__ spans, unsigned long long* grand) {
+k_retain_scan(const u32* __restrict__ qtotal, u32 nq, const u32* __restrict__ n_ptr, u32* __restrict__ qbase, uint2* __restrict__ spans, unsigned long long* grand) {
     __shared__ unsigned long long s_part[1024];
+    if (n_ptr) nq = min(nq, *n_ptr);
     const u32 tid = threadIdx.x;
     const u32 per = (nq + 1023) / 1024;
     const u32 b = min(nq, tid * per), e = min(nq, b + per);
