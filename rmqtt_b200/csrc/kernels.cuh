@@ -176,23 +176,25 @@ __device__ __forceinline__ u32 dict_lookup_inline(const TrieView& tv, const u32 
 }
 
 // (a template only so that every kernel instantiation owns its private out-of-line copy: two kernels sharing one
-//  noinline function made ptxas 12.9 crash once one of them used the bulk-copy / mbarrier instructions)
+//  noinline function made ptxas 12.9 crash once one of them used the bulk-copy / mbarrier instructions).  The table
+//  pointers and the mask come by value: a reference to the kernel's TrieView parameter made every thread copy the whole
+//  view to its stack on entry, long level or not.
 template <int OWNER>
-__device__ __noinline__ u32 dict_lookup_long(const TrieView& tv, const u8* text, u32 len) {
+__device__ __noinline__ u32 dict_lookup_long(const DictSlot* dict, const u8* pool, u32 dict_mask, const u8* text, u32 len) {
     u32 h = FNV_INIT;
     for (u32 i = 0; i < len; ++i) h = fnv_step(h, text[i]);
-    u32 idx = dict_hash_finish(h, len) & tv.dict_mask;
+    u32 idx = dict_hash_finish(h, len) & dict_mask;
     for (;;) {
         u32 s[8];
-        ld256(tv.dict + idx, s);
+        ld256(dict + idx, s);
         if (s[0] == 0) return TOK_UNKNOWN;
         if ((s[7] >> 24) == 0xFFu && s[1] == len && s[3] == h) {
-            const u8* q = tv.pool + s[2];
+            const u8* q = pool + s[2];
             bool eq = true;
             for (u32 i = 0; i < len && eq; ++i) eq = (q[i] == text[i]);
             if (eq) return s[0];
         }
-        idx = (idx + 1) & tv.dict_mask;
+        idx = (idx + 1) & dict_mask;
     }
 }
 
@@ -215,14 +217,16 @@ k_tokenize(const u8* __restrict__ blob, u32 blob_bytes, u32 readable_bytes, cons
     // small-batch graphs: the launch is sized for a CAPACITY `n`; the real batch size and text length sit in device memory
     const u32 stride = n;                        // row stride of the level-major `tok` array
     if (hdr) { n = min(n, hdr[0]); blob_bytes = readable_bytes = hdr[1]; }
-    bool staged = false;
-    u32 sbase = 0;
+    // blob offset of stage byte 0, or NOT_STAGED.  (A separate `staged` flag lived across the barrier as predicate bits that
+    // ptxas spilled to local memory in every thread; the offset is live there anyway.  A staged offset is 16-byte aligned.)
+    constexpr u32 NOT_STAGED = 0xFFFFFFFFu;
+    u32 sbase = NOT_STAGED;
     if (BULK) {
         const u32 t0 = blockIdx.x * TOK_THREADS, t1 = min(n, t0 + TOK_THREADS);
         const bool any = t0 < n;                 // (a capacity-sized launch has CTAs beyond the real batch)
         const u32 b0 = any ? offs[t0] & ~15u : 0u;
         const u32 e0 = any ? (min(offs[t1], blob_bytes) + 15u) & ~15u : 0u;
-        staged = any && sel == nullptr && (reinterpret_cast<uintptr_t>(blob) & 15u) == 0 && e0 > b0 && e0 - b0 <= TOK_STAGE_BYTES && e0 <= readable_bytes;
+        const bool staged = any && sel == nullptr && (reinterpret_cast<uintptr_t>(blob) & 15u) == 0 && e0 > b0 && e0 - b0 <= TOK_STAGE_BYTES && e0 <= readable_bytes;
         if (staged) {           // uniform over the CTA
             sbase = b0;
             if (threadIdx.x == 0) {
@@ -254,7 +258,7 @@ k_tokenize(const u8* __restrict__ blob, u32 blob_bytes, u32 readable_bytes, cons
 #pragma unroll
         for (int k = 0; k < 7; ++k) {
             if (!ended) {
-                u32 x = (BULK && staged) ? text4_s(s_stage, pos - sbase) : text4(blob + pos, limit);
+                u32 x = (BULK && sbase != NOT_STAGED) ? text4_s(s_stage, pos - sbase) : text4(blob + pos, limit);
                 const u32 z = swar_zero_bytes(x ^ 0x2F2F2F2Fu);                       // '/' bytes
                 u32 nb = z ? static_cast<u32>((__ffs(z) - 1) >> 3) : 4u;             // bytes before the first '/'
                 nb = min(nb, end - pos);                                             // ... and before the end of the topic
@@ -279,7 +283,7 @@ k_tokenize(const u8* __restrict__ blob, u32 blob_bytes, u32 readable_bytes, cons
             if (c0 == '$') { if (lev > 0) invalid = true; else dollar = true; }           // topic.rs:210
             if (!invalid && lev < tok_levels) {
                 if (len <= DICT_INLINE_MAX) { w[6] |= len << 24; tk = dict_lookup_inline(tv, w); }
-                else tk = dict_lookup_long<BULK ? 1 : 0>(tv, blob + start, len);
+                else tk = dict_lookup_long<BULK ? 1 : 0>(tv.dict, tv.pool, tv.dict_mask, blob + start, len);
             }
         }
         if (invalid) break;
