@@ -13,12 +13,14 @@
 #include <cstdlib>
 #include <cstring>
 #include <condition_variable>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <type_traits>
 #include <vector>
 
 #include "../../include/gpumqtt.h"
+#include "cuda_owned.h"
 #include "host_trie.h"
 #include "comm.cuh"
 #include "pipeline.cuh"
@@ -28,52 +30,25 @@
 
 using namespace gm;
 
-namespace {
-
-thread_local std::string g_err;
-
-#define CUDA_TRY(expr)                                                                              \
-    do {                                                                                            \
-        cudaError_t _e = (expr);                                                                    \
-        if (_e != cudaSuccess) {                                                                    \
-            g_err = std::string(#expr) + ": " + cudaGetErrorString(_e);                             \
-            return (_e == cudaErrorNoDevice || _e == cudaErrorInsufficientDriver) ? GM_ERR_NO_DEVICE : GM_ERR_CUDA; \
-        }                                                                                           \
-    } while (0)
-
-struct DevBuf {   // owning device allocation (freed on destruction, also on the early-return error paths)
-    void* p = nullptr;
-    size_t cap = 0;
-    DevBuf() = default;
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
-    DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
-    DevBuf& operator=(DevBuf&& o) noexcept { if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; } return *this; }
-    void* detach() { void* q = p; p = nullptr; cap = 0; return q; }
-    ~DevBuf() { release(); }
-    cudaError_t ensure(size_t bytes, bool keep = false, cudaStream_t s = nullptr) {
-        if (bytes <= cap) return cudaSuccess;
-        size_t ncap = std::max(bytes, cap + cap / 2);
-        ncap = (ncap + 255) & ~size_t(255);
-        void* np = nullptr;
-        cudaError_t e = cudaMalloc(&np, ncap);
-        if (e != cudaSuccess) return e;
-        if (keep && p && cap) { e = cudaMemcpyAsync(np, p, cap, cudaMemcpyDeviceToDevice, s); if (e != cudaSuccess) return e; cudaStreamSynchronize(s); }
-        if (p) cudaFree(p);
-        p = np; cap = ncap;
-        return cudaSuccess;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return static_cast<T*>(p); }
-};
+thread_local std::string gm::g_err;
+void gm::nccl_comm_destroy(ncclComm_t c) { NcclApi::get().CommDestroy(c); }
 
 static_assert(GM_ERR_INVALID_TOPIC == -2, "k_tokenize writes the per-topic status code directly");
 
-}  // namespace
-
-struct SmallGraph;
-static void small_graph_destroy(SmallGraph* g);
 constexpr int GM_SMALL_NOT_APPLICABLE = 1000;     // internal: the small-batch fast path declined, take the pipelined path
+
+// One captured small-batch call (small_graph_match, small_graph_retain): its executable graph and the pinned and device
+// in/out blocks the graph copies between.
+struct SmallGraph {
+    u32 cap_n = 0, cap_blob = 0, cap_out = 0;
+    size_t elem = 0;
+    u64 view_epoch = ~0ull, scratch_sig = 0;
+    GraphExec exec;
+    PinnedBuf h_in, h_out;
+    size_t in_bytes = 0, out_bytes = 0, off_offs = 0, off_trees = 0, off_blob = 0, off_spans = 0, off_status = 0, off_out = 0;
+    DevBuf d_in, d_out;
+    bool warmed = false;
+};
 
 // One match CONTEXT = everything a match call needs besides the (read-only) tables: its own streams, events, kernel
 // scratch and staging buffers.  Host-buffer calls take a free context from the engine's pool, enqueue, RELEASE THE
@@ -81,15 +56,15 @@ constexpr int GM_SMALL_NOT_APPLICABLE = 1000;     // internal: the small-batch f
 // concurrent readers under its RwLock, rmqtt/src/router.rs:166) and a mutation never waits behind a D2H copy.
 struct MatchCtx {
     static constexpr int MAXC = 32;  // chunks per pipelined host call
-    cudaStream_t sc = nullptr, s_h2d = nullptr, s_d2h = nullptr;
-    cudaEvent_t ev_h2d[MAXC] = {}, ev_comp[MAXC] = {};
-    cudaEvent_t ev_done = nullptr;   // after the last kernel of the last match enqueued with this context's scratch
+    Stream sc, s_h2d, s_d2h;
+    Event ev_h2d[MAXC], ev_comp[MAXC];
+    Event ev_done;                   // after the last kernel of the last match enqueued with this context's scratch
     bool recorded = false, busy = false;
-    unsigned long long* h_cur = nullptr;             // pinned: cursor snapshot after every chunk
+    PinnedBuf h_cur;                 // cursor snapshot after every chunk (unsigned long long [MAXC])
     DevBuf d_tok, d_tok8, d_meta, d_slow, d_ctrl, d_gstack, d_gpool, d_sort, d_hist;   // kernel scratch
     DevBuf d_blob, d_offs, d_spans, d_ids, d_status, d_trees;                          // staging of host-buffer calls
     // small-batch fast path: the whole call (H2D, memsets, 5 kernels, D2H) as ONE CUDA-graph launch (see SmallGraph)
-    struct SmallGraph* small[2] = {nullptr, nullptr};
+    std::unique_ptr<SmallGraph> small[2];
     // the scratch pointers a captured graph has baked in: a later, larger call may re-allocate any of them
     u64 scratch_sig() const {
         u64 h = 0x9E3779B97F4A7C15ull;
@@ -97,18 +72,17 @@ struct MatchCtx {
         return h;
     }
     int init() {
-        CUDA_TRY(cudaStreamCreateWithFlags(&sc, cudaStreamNonBlocking));
-        CUDA_TRY(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
-        CUDA_TRY(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
+        CUDA_TRY(cudaStreamCreateWithFlags(sc.put(), cudaStreamNonBlocking));
+        CUDA_TRY(cudaStreamCreateWithFlags(s_h2d.put(), cudaStreamNonBlocking));
+        CUDA_TRY(cudaStreamCreateWithFlags(s_d2h.put(), cudaStreamNonBlocking));
         for (int i = 0; i < MAXC; ++i) {
-            CUDA_TRY(cudaEventCreateWithFlags(&ev_h2d[i], cudaEventDisableTiming));
-            CUDA_TRY(cudaEventCreateWithFlags(&ev_comp[i], cudaEventDisableTiming));
+            CUDA_TRY(cudaEventCreateWithFlags(ev_h2d[i].put(), cudaEventDisableTiming));
+            CUDA_TRY(cudaEventCreateWithFlags(ev_comp[i].put(), cudaEventDisableTiming));
         }
-        CUDA_TRY(cudaEventCreateWithFlags(&ev_done, cudaEventDisableTiming));
-        CUDA_TRY(cudaMallocHost(&h_cur, MAXC * sizeof(unsigned long long)));
+        CUDA_TRY(cudaEventCreateWithFlags(ev_done.put(), cudaEventDisableTiming));
+        CUDA_TRY(h_cur.ensure(MAXC * sizeof(unsigned long long)));
         return GM_OK;
     }
-    void destroy();
 };
 
 struct gm_engine {
@@ -124,31 +98,26 @@ struct gm_engine {
     static constexpr int NCTX = 3;   // host-buffer matches in flight
     MatchCtx ctxs[NCTX];
     MatchCtx devctx;                 // scratch of the device-buffer entry points (they run on the CALLER's stream)
-    cudaStream_t side = nullptr;     // flush
+    Stream side;                     // flush
     static constexpr int MAXC = MatchCtx::MAXC;
     static constexpr int RING = 64;   // per-kernel timing events of the last RING match calls
-    cudaEvent_t ev_flush = nullptr;
-    cudaEvent_t ev_ring[RING][4] = {};
+    Event ev_flush;
+    Event ev_ring[RING][4];
     u64 ring_n = 0;
     u64 view_epoch = 0;               // bumped by every flush that changed what the kernels see
     // device tables
     DevBuf d_edges, d_ranges, d_values, d_dict, d_pool, d_cfilter, d_tree_slots;
     size_t up_ranges = 0, up_values = 0, up_pool = 0, up_edges_slots = 0, up_dict_slots = 0;
     u64 up_values_epoch = 0;
-    // flush staging: patches are gathered into PINNED host memory and scattered by kernels on the side stream —
+    // flush staging: patches are gathered into PINNED host memory (h_arena_) and scattered by kernels on the side stream —
     // the flush never synchronises the host with the device
     DevBuf d_patch;
-    char* h_patch = nullptr; size_t h_patch_cap = 0;
-    cudaEvent_t ev_patch = nullptr;  // the previous flush has consumed h_patch
-    bool patch_pending = false;
-    struct Retired { void* p; u64 gen; };
-    std::vector<Retired> retired;    // table buffers replaced by an epoch swap: freed once every match that could see them is done
-    u64 flush_gen = 0;
+    std::vector<DevBuf> retired;     // table buffers replaced by an epoch swap: freed once every match that could see them is done
     // retained tree (device copy of the flattened arrays) + scratch of the retained lookup
     DevBuf d_rnodes, d_rkids, d_redges, d_rvals;
-    DevBuf d_rfront[2], d_rdescs, d_rctl, d_rq, d_rstage[5];
+    DevBuf d_rfront[2], d_rdescs, d_rctl, d_rq;
     u32 r_cap_items = 1u << 22, r_cap_desc = 1u << 22;   // totals over the RQ slices of each queue
-    struct SmallGraph* rsmall[2] = {nullptr, nullptr};   // small retained lookups as one CUDA-graph launch (small_graph_retain; mu_ret)
+    std::unique_ptr<SmallGraph> rsmall[2];   // small retained lookups as one CUDA-graph launch (small_graph_retain; mu_ret)
     u64 launches = 0;
     // fused gather over peer memory (comm.cuh): one block per rank holding every rank's slab; the peers' blocks are opened by CUDA IPC
     struct Gather : GatherLayout {
@@ -157,12 +126,20 @@ struct gm_engine {
         char* peer[8] = {};
         DevBuf d_ptrs;      // device arrays for k_gather_finish: counts pointers [8], flags pointers [8]
         bool connected = false;
+        Gather& operator=(Gather&&) = default;
+        ~Gather() { close(); }
+        void close() {      // the one teardown of the gather (gm_gather_destroy, the engine's destruction): the peers' blocks, then ours
+            if (!block) return;
+            for (u32 w = 0; w < world; ++w) if (w != rank && peer[w]) cudaIpcCloseMemHandle(peer[w]);
+            cudaFree(block);
+            *this = Gather{};
+        }
     } gather;
     // multi-GPU (comm.cuh): NCCL communicator of the root-hash shards, scratch of the size exchange
-    ncclComm_t comm = nullptr;
+    NcclComm comm;
     u32 comm_rank = 0, comm_world = 1;
     DevBuf d_comm, d_part;
-    unsigned long long* h_comm = nullptr;   // pinned [2 * world + 64]
+    PinnedBuf h_comm;                 // unsigned long long [2 * world + 64]
     // tuning / diagnostics knobs, read from the environment once at creation
     struct Knobs : MatchKnobs { u32 e2e_chunk = 262144; bool small_graphs = true; bool retain_stats = false; bool gather_bcast = false; bool gather_direct = false; } knobs;
     void read_knobs() {
@@ -204,16 +181,13 @@ struct gm_engine {
     std::vector<Swap> swaps_;
     size_t stage_used_ = 0;
     int arena_ = 0;
-    char* h_arena_[2] = {nullptr, nullptr}; size_t h_arena_cap_[2] = {0, 0};
-    cudaEvent_t ev_arena_[2] = {nullptr, nullptr}; bool arena_pending_[2] = {false, false};
+    PinnedBuf h_arena_[2];
+    Event ev_arena_[2]; bool arena_pending_[2] = {false, false};
 
     int stage_reserve(size_t bytes) {
-        if (bytes <= h_arena_cap_[arena_]) return GM_OK;
-        size_t ncap = std::max(bytes, h_arena_cap_[arena_] * 2 + (size_t(1) << 20));
-        char* np = nullptr;
-        CUDA_TRY(cudaMallocHost(&np, ncap));
-        if (h_arena_[arena_]) { std::memcpy(np, h_arena_[arena_], stage_used_); cudaFreeHost(h_arena_[arena_]); }
-        h_arena_[arena_] = np; h_arena_cap_[arena_] = ncap;
+        PinnedBuf& a = h_arena_[arena_];
+        if (bytes <= a.cap) return GM_OK;
+        CUDA_TRY(a.ensure(std::max(bytes, a.cap * 2 + (size_t(1) << 20)), stage_used_));
         return GM_OK;
     }
 
@@ -228,9 +202,8 @@ struct gm_engine {
         if (nd == 0) return GM_OK;
         const size_t off_idx = (stage_used_ + 31) & ~size_t(31);
         const size_t off_data = (off_idx + nd * sizeof(u32) + 31) & ~size_t(31);
-        int st = stage_reserve(off_data + nd * sizeof(T));
-        if (st != GM_OK) return st;
-        char* base = h_arena_[arena_];
+        GM_TRY(stage_reserve(off_data + nd * sizeof(T)));
+        char* base = h_arena_[arena_].p;
         std::memcpy(base + off_idx, dirty.data(), nd * sizeof(u32));
         T* data = reinterpret_cast<T*>(base + off_data);
         for (u32 i = 0; i < nd; ++i) data[i] = host[dirty[i]];
@@ -271,8 +244,7 @@ struct gm_engine {
         using T = std::remove_cv_t<std::remove_reference_t<decltype(host[0])>>;
         const size_t bytes = host.size() * sizeof(T);
         if (ship_appendable_fresh(up, bytes, buf.p != nullptr, buf.cap)) {
-            int st = stage_fresh(buf, host, appendable_room(bytes));
-            if (st != GM_OK) return st;
+            GM_TRY(stage_fresh(buf, host, appendable_room(bytes)));
             up = host.size();
             if (dirty) dirty->clear();
             return GM_OK;
@@ -284,8 +256,7 @@ struct gm_engine {
         }
         if (dirty) {
             dirty->erase(std::remove_if(dirty->begin(), dirty->end(), [&](u32 i) { return i >= before; }), dirty->end());
-            int st = stage_patches(buf, host, *dirty);
-            if (st != GM_OK) return st;
+            GM_TRY(stage_patches(buf, host, *dirty));
             dirty->clear();
         }
         return GM_OK;
@@ -294,7 +265,6 @@ struct gm_engine {
     void free_retired(bool all) {
         if (retired.empty()) return;
         if (!all && cudaEventQuery(ev_flush) != cudaSuccess) return;     // the last fence has not passed yet: some match may still read them
-        for (const Retired& r : retired) cudaFree(r.p);
         retired.clear();
     }
 
@@ -328,49 +298,48 @@ struct gm_engine {
         arena_ ^= 1;
         if (arena_pending_[arena_]) { CUDA_TRY(cudaEventSynchronize(ev_arena_[arena_])); arena_pending_[arena_] = false; }   // two flushes ago: long done
         jobs_.clear(); swaps_.clear(); stage_used_ = 0;
-        int rs;
         bool r_shipped = false;
         if (rtree.dirty) {   // retained tree: whole arrays after a (re)flatten, else only the entries set / remove edited in place
             rtree.prepare_flush();
             if (rtree.full) {
                 const std::vector<u32> marker{0u};       // "retained tree shipped" (records travel in rkids / redges)
-                if ((rs = stage_fresh(d_rnodes, marker, 0)) != GM_OK) return rs;
-                if ((rs = stage_fresh(d_rkids, rtree.rkids, 0, retained_kids_slack(rtree.rkids.size()))) != GM_OK) return rs;
-                if ((rs = stage_fresh(d_redges, rtree.redges, 0)) != GM_OK) return rs;
-                if ((rs = stage_fresh(d_rvals, rtree.rvals, 0, RETAINED_VALS_SLACK)) != GM_OK) return rs;
+                GM_TRY(stage_fresh(d_rnodes, marker, 0));
+                GM_TRY(stage_fresh(d_rkids, rtree.rkids, 0, retained_kids_slack(rtree.rkids.size())));
+                GM_TRY(stage_fresh(d_redges, rtree.redges, 0));
+                GM_TRY(stage_fresh(d_rvals, rtree.rvals, 0, RETAINED_VALS_SLACK));
                 up_rkids = rtree.rkids.size(); up_rvals = rtree.rvals.size(); up_redges_slots = rtree.redges.size();
             } else {
                 bool full_edges = false;
-                if ((rs = upload_appendable(d_rkids, rtree.rkids, up_rkids, &rtree.dirty_kids)) != GM_OK) return rs;
-                if ((rs = upload_table(d_redges, rtree.redges, full_edges, rtree.dirty_edges, up_redges_slots)) != GM_OK) return rs;
-                if ((rs = upload_appendable(d_rvals, rtree.rvals, up_rvals, &rtree.dirty_vals)) != GM_OK) return rs;
+                GM_TRY(upload_appendable(d_rkids, rtree.rkids, up_rkids, &rtree.dirty_kids));
+                GM_TRY(upload_table(d_redges, rtree.redges, full_edges, rtree.dirty_edges, up_redges_slots));
+                GM_TRY(upload_appendable(d_rvals, rtree.rvals, up_rvals, &rtree.dirty_vals));
             }
             r_shipped = true;
         }
-        if ((rs = upload_table(d_edges, trie.edges, trie.full_edges, trie.dirty_edges, up_edges_slots)) != GM_OK) return rs;
-        if ((rs = upload_table(d_dict, trie.dict, trie.full_dict, trie.dirty_dict, up_dict_slots)) != GM_OK) return rs;
-        if ((rs = upload_appendable(d_ranges, trie.ranges, up_ranges, nullptr)) != GM_OK) return rs;
-        if ((rs = upload_appendable(d_values, trie.values, up_values, nullptr)) != GM_OK) return rs;
-        if ((rs = upload_appendable(d_pool, trie.pool, up_pool, nullptr)) != GM_OK) return rs;
+        GM_TRY(upload_table(d_edges, trie.edges, trie.full_edges, trie.dirty_edges, up_edges_slots));
+        GM_TRY(upload_table(d_dict, trie.dict, trie.full_dict, trie.dirty_dict, up_dict_slots));
+        GM_TRY(upload_appendable(d_ranges, trie.ranges, up_ranges, nullptr));
+        GM_TRY(upload_appendable(d_values, trie.values, up_values, nullptr));
+        GM_TRY(upload_appendable(d_pool, trie.pool, up_pool, nullptr));
         if (trie.cfilter_dirty) {   // child filter of wide nodes: a few MB, shipped whole into a new buffer (a rebuild changes its geometry)
-            if ((rs = stage_fresh(d_cfilter, trie.cfilter, 0)) != GM_OK) return rs;
+            GM_TRY(stage_fresh(d_cfilter, trie.cfilter, 0));
             trie.cfilter_dirty = false;
         }
         if (trie.trees_dirty) {      // root records of the extra trees (ACL rules, rewrite rules, ...): a tiny array, shipped whole
-            if ((rs = stage_fresh(d_tree_slots, trie.tree_slots, 0)) != GM_OK) return rs;
+            GM_TRY(stage_fresh(d_tree_slots, trie.tree_slots, 0));
             trie.trees_dirty = false;
         }
         trie.root_dirty = false;
         if (stage_used_) {
             CUDA_TRY(d_patch.ensure(stage_used_));
-            CUDA_TRY(cudaMemcpyAsync(d_patch.p, h_arena_[arena_], stage_used_, cudaMemcpyHostToDevice, side));
+            CUDA_TRY(cudaMemcpyAsync(d_patch.p, h_arena_[arena_].p, stage_used_, cudaMemcpyHostToDevice, side));
         }
         // ---------------- phase B: the fence ----------------
         {
             std::lock_guard<std::mutex> gd(mu_dev);
             for (MatchCtx* c : all_ctxs()) if (c->recorded) CUDA_TRY(cudaStreamWaitEvent(side, c->ev_done, 0));   // never patch under a running match
             for (Swap& sw : swaps_) {
-                if (sw.dst->p) retired.push_back(Retired{sw.dst->detach(), flush_gen});
+                if (sw.dst->p) retired.push_back(std::move(*sw.dst));
                 *sw.dst = std::move(sw.fresh);
             }
             swaps_.clear();
@@ -391,7 +360,6 @@ struct gm_engine {
             dev_rview = retain_view(rtree, d_rkids.as<RKid>(), d_redges.as<REdge>(), d_rvals.as<u32>());
             view_epoch++;
             CUDA_TRY(cudaEventRecord(ev_flush, side));
-            flush_gen++;
         }
         if (r_shipped) rtree.shipped();
         return GM_OK;
@@ -431,7 +399,7 @@ struct gm_engine {
         m.tok = c.d_tok.as<u32>(); m.tok8 = c.d_tok8.as<u32>(); m.meta = c.d_meta.as<u32>(); m.slow = c.d_slow.as<u32>(); m.sort = c.d_sort.as<u32>(); m.hist = c.d_hist.as<u32>();
         m.ctrl = c.d_ctrl.as<Ctrl>(); m.gstack = c.d_gstack.as<u64>(); m.gpool = c.d_gpool.as<Desc>();
         for (const ByteRange& r : match_resets(p, m, a.keep_cursor).r) CUDA_TRY(cudaMemsetAsync(r.p, 0, r.bytes, s));
-        cudaEvent_t* ev_t = ev_ring[ring_n % RING];
+        const Event* ev_t = ev_ring[ring_n % RING];
         cudaError_t ev = cudaSuccess;
         launch_match(p, m, a, kn, dev_view, s, [&](int k) { if (a.timing && ev == cudaSuccess) ev = cudaEventRecord(ev_t[k], s); });
         CUDA_TRY(ev);
@@ -475,8 +443,7 @@ struct gm_engine {
         MatchCtx& c = devctx;
         const RetainPlan p = plan_retain(static_cast<u32>(n), dev_rview.max_depth, r_cap_items, r_cap_desc, num_sms);
         RetainScratch r;
-        int st = retain_scratch(p, r);
-        if (st != GM_OK) return st;
+        GM_TRY(retain_scratch(p, r));
         if (!hdr) {
             CUDA_TRY(cudaStreamWaitEvent(s, ev_flush, 0));
             if (c.recorded) CUDA_TRY(cudaStreamWaitEvent(s, c.ev_done, 0));
@@ -484,7 +451,7 @@ struct gm_engine {
         CUDA_TRY(cudaMemsetAsync(d_rctl.p, 0, p.ctl, s));
         CUDA_TRY(cudaMemsetAsync(d_rq.p, 0, p.rq, s));
         const bool timing = hdr == nullptr;
-        cudaEvent_t* ev_t = ev_ring[ring_n % RING];
+        const Event* ev_t = ev_ring[ring_n % RING];
         cudaError_t ev = cudaSuccess;
         launch_retain(p, r, dev_view, dev_rview, d_blob_, blob_bytes, d_offs_, d_spans_, d_ids_, cap_ids, d_status_, knobs.retain_stats && !hdr, s, hdr,
                       [&](int k) { if (timing && ev == cudaSuccess) ev = cudaEventRecord(ev_t[k], s); });
@@ -502,8 +469,7 @@ struct gm_engine {
     // runs the pipeline, growing the frontier / descriptor scratch until nothing overflowed; leaves *total
     int run_retain(const void* d_blob_, u64 blob_bytes, const u32* d_offs_, u64 n, gm_span* d_spans_, u32* d_ids_, u64 cap_ids, int32_t* d_status_, cudaStream_t s, u64* total) {
         for (int attempt = 0; attempt < 12; ++attempt) {
-            int st = enqueue_retain(d_blob_, blob_bytes, d_offs_, n, d_spans_, d_ids_, cap_ids, d_status_, s);
-            if (st != GM_OK) return st;
+            GM_TRY(enqueue_retain(d_blob_, blob_bytes, d_offs_, n, d_spans_, d_ids_, cap_ids, d_status_, s));
             RCtl h{};
             CUDA_TRY(cudaMemcpyAsync(&h, d_rctl.p, sizeof(RCtl), cudaMemcpyDeviceToHost, s));
             CUDA_TRY(cudaStreamSynchronize(s));
@@ -552,19 +518,18 @@ int32_t gm_create(const gm_config* cfg, gm_engine** out) {
     if (dev < 0) CUDA_TRY(cudaGetDevice(&dev));
     if (dev >= ndev) { g_err = "device ordinal out of range"; return GM_ERR_INVALID_ARG; }
     CUDA_TRY(cudaSetDevice(dev));
-    gm_engine* eng = new gm_engine(c.max_levels ? c.max_levels : 128u);
-    struct Guard { gm_engine* e; ~Guard() { if (e) gm_destroy(e); } } guard{eng};   // a failing CUDA call below must not leak the half-built engine
+    std::unique_ptr<gm_engine> eng(new gm_engine(c.max_levels ? c.max_levels : 128u));   // a failing CUDA call below frees the half-built engine
     eng->device = dev;
     eng->flags = c.flags;
     eng->read_knobs();
     cudaDeviceProp prop{};
     CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
     eng->num_sms = prop.multiProcessorCount;
-    CUDA_TRY(cudaStreamCreateWithFlags(&eng->side, cudaStreamNonBlocking));
-    for (MatchCtx* cx : eng->all_ctxs()) { int st = cx->init(); if (st != GM_OK) return st; }
-    CUDA_TRY(cudaEventCreateWithFlags(&eng->ev_flush, cudaEventDisableTiming));
-    for (auto& ev : eng->ev_arena_) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    for (auto& q : eng->ev_ring) for (auto& ev : q) CUDA_TRY(cudaEventCreate(&ev));
+    CUDA_TRY(cudaStreamCreateWithFlags(eng->side.put(), cudaStreamNonBlocking));
+    for (MatchCtx* cx : eng->all_ctxs()) GM_TRY(cx->init());
+    CUDA_TRY(cudaEventCreateWithFlags(eng->ev_flush.put(), cudaEventDisableTiming));
+    for (auto& ev : eng->ev_arena_) CUDA_TRY(cudaEventCreateWithFlags(ev.put(), cudaEventDisableTiming));
+    for (auto& q : eng->ev_ring) for (auto& ev : q) CUDA_TRY(cudaEventCreate(ev.put()));
     CUDA_TRY(cudaEventRecord(eng->ev_flush, eng->side));
     for (auto k : {k2_kernel(false, false, false), k2_kernel(false, true, false), k2_kernel(true, false, false), k2_kernel(true, true, false), k2_kernel(false, false, true)})
         CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, int(K2_SMEM)));
@@ -574,44 +539,18 @@ int32_t gm_create(const gm_config* cfg, gm_engine** out) {
     if (const char* ev = getenv("GM_L2_FETCH")) { const int v = atoi(ev); if (v == 32 || v == 64 || v == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, static_cast<size_t>(v)); }
     else if (c.flags & GM_FLAG_L2_FETCH_32) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
     if (c.filters_hint) eng->trie.reserve(c.filters_hint);
-    guard.e = nullptr;
-    *out = eng;
+    *out = eng.release();
     return GM_OK;
 }
 
-void MatchCtx::destroy() {
-    for (DevBuf* b : {&d_tok, &d_tok8, &d_meta, &d_slow, &d_ctrl, &d_gstack, &d_gpool, &d_sort, &d_hist, &d_blob, &d_offs, &d_spans, &d_ids, &d_status, &d_trees}) b->release();
-    for (auto& g : small) if (g) { small_graph_destroy(g); g = nullptr; }
-    if (sc) cudaStreamDestroy(sc);
-    if (s_h2d) cudaStreamDestroy(s_h2d);
-    if (s_d2h) cudaStreamDestroy(s_d2h);
-    for (int i = 0; i < MAXC; ++i) { if (ev_h2d[i]) cudaEventDestroy(ev_h2d[i]); if (ev_comp[i]) cudaEventDestroy(ev_comp[i]); }
-    if (ev_done) cudaEventDestroy(ev_done);
-    if (h_cur) cudaFreeHost(h_cur);
-}
-
+// every resource of the engine is released by its owner; what is left here is to wait for the device first
 void gm_destroy(gm_engine* e) {
     if (!e) return;
-    if (e->flags & GM_FLAG_HOST_ONLY) { delete e; return; }
-    cudaSetDevice(e->device);
-    cudaDeviceSynchronize();
-    e->free_retired(true);
-    for (MatchCtx* cx : e->all_ctxs()) cx->destroy();
-    for (auto& g : e->rsmall) if (g) { small_graph_destroy(g); g = nullptr; }
-    for (DevBuf* b : {&e->d_cfilter, &e->d_tree_slots, &e->d_edges, &e->d_ranges, &e->d_values, &e->d_dict, &e->d_pool, &e->d_patch, &e->d_rnodes, &e->d_rkids, &e->d_redges,
-                      &e->d_rvals, &e->d_rfront[0], &e->d_rfront[1], &e->d_rdescs, &e->d_rctl, &e->d_rq, &e->d_rstage[0], &e->d_rstage[1], &e->d_rstage[2],
-                      &e->d_rstage[3], &e->d_rstage[4]})
-        b->release();
-    if (e->side) cudaStreamDestroy(e->side);
-    if (e->comm) { NcclApi::get().CommDestroy(e->comm); e->comm = nullptr; }
-    if (e->h_comm) cudaFreeHost(e->h_comm);
-    e->d_comm.release(); e->d_part.release();
-    if (e->gather.block) { for (u32 w = 0; w < e->gather.world; ++w) if (w != e->gather.rank && e->gather.peer[w]) cudaIpcCloseMemHandle(e->gather.peer[w]); cudaFree(e->gather.block); e->gather.block = nullptr; }
-    e->gather.d_ptrs.release();
-    for (auto& hp : e->h_arena_) if (hp) cudaFreeHost(hp);
-    for (auto& ev : e->ev_arena_) if (ev) cudaEventDestroy(ev);
-    if (e->ev_flush) cudaEventDestroy(e->ev_flush);
-    for (auto& q : e->ev_ring) for (auto& ev : q) if (ev) cudaEventDestroy(ev);
+    if (!(e->flags & GM_FLAG_HOST_ONLY)) {
+        cudaSetDevice(e->device);
+        cudaDeviceSynchronize();
+        e->free_retired(true);
+    }
     delete e;
 }
 
@@ -705,7 +644,7 @@ static int32_t match_device_impl(gm_engine* e, const void* d_blob, uint64_t blob
     if (blob_bytes > 0xFFFFFFFFull) { g_err = "topic blob >= 4 GiB"; return GM_ERR_TOO_LARGE; }
     if (e->flags & GM_FLAG_HOST_ONLY) { g_err = "host-only engine cannot match: there is no CPU fallback"; return GM_ERR_NO_DEVICE; }
     CUDA_TRY(cudaSetDevice(e->device));
-    { int st = auto_flush(e); if (st != GM_OK) return st; }
+    GM_TRY(auto_flush(e));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     std::unique_lock<std::mutex> gd(e->mu_dev);
     gm_engine::MatchCall a;
@@ -763,23 +702,6 @@ int32_t gm_match_batch_device_ex(gm_engine* e, const gm_match_args* a) {
 // cudaGraphLaunch, wait for one event, copy the results out of the pinned out-block.  The kernels carry the table view
 // by value, so the graph is re-captured (cudaGraphExecUpdate) when a flush has changed the view.  Small retained lookups
 // (small_graph_retain) use the same tiers, blocks and capture helper.
-struct SmallGraph {
-    u32 cap_n = 0, cap_blob = 0, cap_out = 0;
-    size_t elem = 0;
-    u64 view_epoch = ~0ull, scratch_sig = 0;
-    cudaGraphExec_t exec = nullptr;
-    char *h_in = nullptr, *h_out = nullptr;
-    size_t in_bytes = 0, out_bytes = 0, off_offs = 0, off_trees = 0, off_blob = 0, off_spans = 0, off_status = 0, off_out = 0;
-    DevBuf d_in, d_out;
-    bool warmed = false;
-};
-static void small_graph_destroy(SmallGraph* g) {
-    if (!g) return;
-    if (g->exec) cudaGraphExecDestroy(g->exec);
-    if (g->h_in) cudaFreeHost(g->h_in);
-    if (g->h_out) cudaFreeHost(g->h_out);
-    delete g;
-}
 
 // Capacity tiers: tier 0 holds up to 64 rows and 8 KiB of text, tier 1 up to 2048 rows and 192 KiB; their outputs hold
 // 4096 and 128 K elements (ids, or 8-byte descriptors).  -1: the batch is larger than both.
@@ -791,18 +713,19 @@ static int small_graph_tier(u64 n, u64 blob_bytes) {
 
 // in-block:  {n, text bytes} (16 B) | offsets [cap_n + 1] | trees [cap_n] | text (256-aligned)
 // out-block: head (32 B: the match's cursor, or the retained lookup's RCtl head) | spans [cap_n] | status [cap_n] | output (256-aligned)
-static int small_graph_new(SmallGraph*& g, int tier) {
-    g = new SmallGraph();
+static int small_graph_new(std::unique_ptr<SmallGraph>& slot, int tier) {
+    auto g = std::make_unique<SmallGraph>();
     g->cap_n = tier == 0 ? 64u : 2048u; g->cap_blob = tier == 0 ? 8u * 1024u : 192u * 1024u; g->cap_out = tier == 0 ? 4096u : 128u * 1024u;
     g->off_offs = 16; g->off_trees = g->off_offs + (g->cap_n + 1) * sizeof(u32); g->off_blob = (g->off_trees + g->cap_n * sizeof(u32) + 255) & ~size_t(255);
     g->in_bytes = g->off_blob + g->cap_blob + 32;
     g->off_spans = 32; g->off_status = g->off_spans + g->cap_n * sizeof(gm_span); g->off_out = (g->off_status + g->cap_n * sizeof(int32_t) + 255) & ~size_t(255);
     g->out_bytes = g->off_out + static_cast<size_t>(g->cap_out) * 8;
-    CUDA_TRY(cudaMallocHost(&g->h_in, g->in_bytes));
-    CUDA_TRY(cudaMallocHost(&g->h_out, g->out_bytes));
+    CUDA_TRY(g->h_in.ensure(g->in_bytes));
+    CUDA_TRY(g->h_out.ensure(g->out_bytes));
     CUDA_TRY(g->d_in.ensure(g->in_bytes));
     CUDA_TRY(g->d_out.ensure(g->out_bytes));
-    std::memset(g->h_in, 0, g->in_bytes);
+    std::memset(g->h_in.p, 0, g->in_bytes);
+    slot = std::move(g);
     return GM_OK;
 }
 
@@ -814,18 +737,19 @@ static int small_graph_refresh(SmallGraph* g, cudaStream_t s, u64 view_epoch, u6
     if (g->exec && g->view_epoch == view_epoch && g->elem == elem && g->scratch_sig == scratch_sig) return GM_OK;
     cudaGraph_t graph = nullptr;
     CUDA_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-    cudaError_t ce = cudaMemcpyAsync(g->d_in.p, g->h_in, g->in_bytes, cudaMemcpyHostToDevice, s);
+    cudaError_t ce = cudaMemcpyAsync(g->d_in.p, g->h_in.p, g->in_bytes, cudaMemcpyHostToDevice, s);
     int st = ce == cudaSuccess ? enqueue(s) : GM_ERR_CUDA;
-    if (st == GM_OK) ce = cudaMemcpyAsync(g->h_out, g->d_out.p, g->out_bytes, cudaMemcpyDeviceToHost, s);
+    if (st == GM_OK) ce = cudaMemcpyAsync(g->h_out.p, g->d_out.p, g->out_bytes, cudaMemcpyDeviceToHost, s);
     cudaError_t ee = cudaStreamEndCapture(s, &graph);
     if (st != GM_OK || ce != cudaSuccess || ee != cudaSuccess) { if (graph) cudaGraphDestroy(graph); g_err = "small-batch graph capture failed"; return st != GM_OK ? st : GM_ERR_CUDA; }
     bool ok = false;
     if (g->exec) {
         cudaGraphExecUpdateResultInfo info{};
         ok = cudaGraphExecUpdate(g->exec, graph, &info) == cudaSuccess;
-        if (!ok) { cudaGetLastError(); cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
+        if (!ok) { cudaGetLastError(); g->exec.reset(); }
     }
-    if (!ok) { const cudaError_t ie = cudaGraphInstantiate(&g->exec, graph, 0); if (ie != cudaSuccess) { cudaGraphDestroy(graph); g->exec = nullptr; CUDA_TRY(ie); } }
+    cudaGraphExec_t exec = nullptr;
+    if (!ok) { const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0); if (ie != cudaSuccess) { cudaGraphDestroy(graph); CUDA_TRY(ie); } g->exec.reset(exec); }
     cudaGraphDestroy(graph);
     g->view_epoch = view_epoch; g->elem = elem; g->scratch_sig = scratch_sig;
     return GM_OK;
@@ -834,19 +758,20 @@ static int small_graph_refresh(SmallGraph* g, cudaStream_t s, u64 view_epoch, u6
 // fill the pinned in-block: {n, text bytes} | offsets re-based to 0 | text
 static void small_graph_fill(SmallGraph* g, const char* blob, const uint32_t* offsets, uint64_t n) {
     const u64 b0 = offsets[0], blob_bytes = offsets[n] - b0;
-    u32* hdr = reinterpret_cast<u32*>(g->h_in);
+    u32* hdr = reinterpret_cast<u32*>(g->h_in.p);
     hdr[0] = static_cast<u32>(n); hdr[1] = static_cast<u32>(blob_bytes);
-    u32* ho = reinterpret_cast<u32*>(g->h_in + g->off_offs);
+    u32* ho = reinterpret_cast<u32*>(g->h_in.p + g->off_offs);
     for (u64 i = 0; i <= n; ++i) ho[i] = static_cast<u32>(offsets[i] - b0);
-    if (blob_bytes) std::memcpy(g->h_in + g->off_blob, blob + b0, blob_bytes);
+    if (blob_bytes) std::memcpy(g->h_in.p + g->off_blob, blob + b0, blob_bytes);
 }
 
 static int small_graph_match(gm_engine* e, MatchCtx& c, std::unique_lock<std::mutex>& gd, const char* blob, const uint32_t* offsets, uint64_t n,
                              gm_span* out_spans, void* out, size_t elem, uint64_t cap_user, uint64_t* needed, int32_t* status, const uint32_t* trees) {
     const int tier = small_graph_tier(n, offsets[n] - offsets[0]);
     if (tier < 0) return GM_SMALL_NOT_APPLICABLE;
-    SmallGraph*& g = c.small[tier];
-    if (!g) { int st = small_graph_new(g, tier); if (st != GM_OK) return st; }
+    std::unique_ptr<SmallGraph>& slot = c.small[tier];
+    if (!slot) GM_TRY(small_graph_new(slot, tier));
+    SmallGraph* g = slot.get();
     const bool desc = elem == 8;
     auto enqueue = [&](cudaStream_t s) -> int {
         char* di = static_cast<char*>(g->d_in.p);
@@ -860,20 +785,18 @@ static int small_graph_match(gm_engine* e, MatchCtx& c, std::unique_lock<std::mu
     };
     if (!g->warmed) {      // allocate the scratch and set kernel attributes outside any capture: one empty (n = 0) pass
         CUDA_TRY(cudaMemsetAsync(g->d_in.p, 0, g->in_bytes, c.sc));
-        int st = enqueue(c.sc);
-        if (st != GM_OK) return st;
+        GM_TRY(enqueue(c.sc));
         CUDA_TRY(cudaStreamSynchronize(c.sc));
         g->warmed = true;
     }
     if (g->exec && g->scratch_sig != c.scratch_sig()) {      // a larger call re-allocated this context's scratch since the capture:
         CUDA_TRY(cudaMemsetAsync(g->d_in.p, 0, g->in_bytes, c.sc));   // size it again (empty pass), then re-capture with the new pointers
-        int st = enqueue(c.sc);
-        if (st != GM_OK) return st;
+        GM_TRY(enqueue(c.sc));
         CUDA_TRY(cudaStreamSynchronize(c.sc));
     }
-    { int st = small_graph_refresh(g, c.sc, e->view_epoch, c.scratch_sig(), elem, enqueue); if (st != GM_OK) return st; }
+    GM_TRY(small_graph_refresh(g, c.sc, e->view_epoch, c.scratch_sig(), elem, enqueue));
     small_graph_fill(g, blob, offsets, n);
-    if (trees) std::memcpy(g->h_in + g->off_trees, trees, n * sizeof(u32)); else std::memset(g->h_in + g->off_trees, 0, n * sizeof(u32));
+    if (trees) std::memcpy(g->h_in.p + g->off_trees, trees, n * sizeof(u32)); else std::memset(g->h_in.p + g->off_trees, 0, n * sizeof(u32));
     CUDA_TRY(cudaStreamWaitEvent(c.sc, e->ev_flush, 0));
     CUDA_TRY(cudaGraphLaunch(g->exec, c.sc));
     CUDA_TRY(cudaEventRecord(c.ev_done, c.sc));
@@ -881,13 +804,13 @@ static int small_graph_match(gm_engine* e, MatchCtx& c, std::unique_lock<std::mu
     e->launches += desc ? 5 : 6;
     gd.unlock();
     CUDA_TRY(cudaEventSynchronize(c.ev_done));
-    const u64 total = *reinterpret_cast<const u64*>(g->h_out);
+    const u64 total = *reinterpret_cast<const u64*>(g->h_out.p);
     if (total > g->cap_out) return GM_SMALL_NOT_APPLICABLE;      // more output than the tier holds: the pipelined path handles it
     if (needed) *needed = total;
-    std::memcpy(status, g->h_out + g->off_status, n * sizeof(int32_t));
+    std::memcpy(status, g->h_out.p + g->off_status, n * sizeof(int32_t));
     if (total > cap_user) { g_err = "output buffer too small"; return GM_ERR_CAPACITY; }
-    std::memcpy(out_spans, g->h_out + g->off_spans, n * sizeof(gm_span));
-    if (total) std::memcpy(out, g->h_out + g->off_out, total * elem);
+    std::memcpy(out_spans, g->h_out.p + g->off_spans, n * sizeof(gm_span));
+    if (total) std::memcpy(out, g->h_out.p + g->off_out, total * elem);
     return GM_OK;
 }
 
@@ -902,8 +825,9 @@ static int small_graph_retain(gm_engine* e, const char* blob, const uint32_t* of
                               uint64_t* needed, int32_t* status) {
     const int tier = small_graph_tier(n, offsets[n] - offsets[0]);
     if (tier < 0) return GM_SMALL_NOT_APPLICABLE;
-    SmallGraph*& g = e->rsmall[tier];
-    if (!g) { int st = small_graph_new(g, tier); if (st != GM_OK) return st; }
+    std::unique_ptr<SmallGraph>& slot = e->rsmall[tier];
+    if (!slot) GM_TRY(small_graph_new(slot, tier));
+    SmallGraph* g = slot.get();
     MatchCtx& c = e->devctx;
     std::unique_lock<std::mutex> gd(e->mu_dev);
     auto enqueue = [&](cudaStream_t s) -> int {
@@ -935,9 +859,9 @@ static int small_graph_retain(gm_engine* e, const char* blob, const uint32_t* of
         }
         if (st != GM_OK) return st;
     }
-    { int st = small_graph_refresh(g, c.sc, e->view_epoch, e->retain_sig(), sizeof(u32), enqueue); if (st != GM_OK) return st; }
+    GM_TRY(small_graph_refresh(g, c.sc, e->view_epoch, e->retain_sig(), sizeof(u32), enqueue));
     small_graph_fill(g, blob, offsets, n);
-    { int st = order(); if (st != GM_OK) return st; }
+    GM_TRY(order());
     CUDA_TRY(cudaGraphLaunch(g->exec, c.sc));
     CUDA_TRY(cudaEventRecord(c.ev_done, c.sc));
     c.recorded = true;
@@ -945,13 +869,13 @@ static int small_graph_retain(gm_engine* e, const char* blob, const uint32_t* of
     gd.unlock();
     CUDA_TRY(cudaStreamSynchronize(c.sc));
     RCtl head;
-    std::memcpy(static_cast<void*>(&head), g->h_out, offsetof(RCtl, err) + sizeof(u32));
+    std::memcpy(static_cast<void*>(&head), g->h_out.p, offsetof(RCtl, err) + sizeof(u32));
     if (head.err != 0 || head.grand > g->cap_out) return GM_SMALL_NOT_APPLICABLE;
     if (needed) *needed = head.grand;
-    std::memcpy(status, g->h_out + g->off_status, n * sizeof(int32_t));
-    std::memcpy(out_spans, g->h_out + g->off_spans, n * sizeof(gm_span));
+    std::memcpy(status, g->h_out.p + g->off_status, n * sizeof(int32_t));
+    std::memcpy(out_spans, g->h_out.p + g->off_spans, n * sizeof(gm_span));
     if (head.grand > cap_ids) { g_err = "out_ids too small"; return GM_ERR_CAPACITY; }
-    if (head.grand) std::memcpy(out_ids, g->h_out + g->off_out, head.grand * sizeof(u32));
+    if (head.grand) std::memcpy(out_ids, g->h_out.p + g->off_out, head.grand * sizeof(u32));
     return GM_OK;
 }
 
@@ -984,7 +908,7 @@ static int32_t match_host_impl(gm_engine* e, const char* blob, const uint32_t* o
     const bool desc = elem == 8;
     if (e->flags & GM_FLAG_HOST_ONLY) { g_err = "host-only engine cannot match: there is no CPU fallback"; return GM_ERR_NO_DEVICE; }
     CUDA_TRY(cudaSetDevice(e->device));
-    { int st = auto_flush(e); if (st != GM_OK) return st; }
+    GM_TRY(auto_flush(e));
     const u64 blob_bytes = offsets[n];
     if (cap_ids > 0xFFFFFFFFull) cap_ids = 0xFFFFFFFFull;
     CtxLease lease(e);
@@ -1023,9 +947,8 @@ static int32_t match_host_impl(gm_engine* e, const char* blob, const uint32_t* o
         a.blob = c.d_blob.p; a.blob_bytes = offsets[c1]; a.readable_bytes = (offsets[c1] + 15) & ~u64(15); a.offs = c.d_offs.as<u32>() + c0; a.n = c1 - c0;
         a.trees = trees ? c.d_trees.as<u32>() + c0 : nullptr;
         a.spans = c.d_spans.as<gm_span>() + c0; a.out = c.d_ids.p; a.cap = cap_ids; a.status = c.d_status.as<int32_t>() + c0; a.desc = desc; a.keep_cursor = k != 0;
-        int st = e->enqueue_match(c, a, c.sc);
-        if (st != GM_OK) return st;
-        CUDA_TRY(cudaMemcpyAsync(&c.h_cur[k], &c.d_ctrl.as<Ctrl>()->cursor, sizeof(u64), cudaMemcpyDeviceToHost, c.sc));
+        GM_TRY(e->enqueue_match(c, a, c.sc));
+        CUDA_TRY(cudaMemcpyAsync(&c.h_cur.as<unsigned long long>()[k], &c.d_ctrl.as<Ctrl>()->cursor, sizeof(u64), cudaMemcpyDeviceToHost, c.sc));
         CUDA_TRY(cudaEventRecord(c.ev_comp[k], c.sc));
     }
     gd.unlock();        // everything is enqueued: other calls (and flushes) proceed while this one waits for its copies
@@ -1033,7 +956,7 @@ static int32_t match_host_impl(gm_engine* e, const char* blob, const uint32_t* o
     for (int k = 0; k < nchunks; ++k) {
         const u64 c0 = k * chunk, c1 = std::min<u64>(n, c0 + chunk);
         CUDA_TRY(cudaEventSynchronize(c.ev_comp[k]));
-        const u64 cur = c.h_cur[k];
+        const u64 cur = c.h_cur.as<unsigned long long>()[k];
         CUDA_TRY(cudaMemcpyAsync(out_spans + c0, c.d_spans.as<gm_span>() + c0, (c1 - c0) * sizeof(gm_span), cudaMemcpyDeviceToHost, c.s_d2h));
         CUDA_TRY(cudaMemcpyAsync(status + c0, c.d_status.as<int32_t>() + c0, (c1 - c0) * sizeof(int32_t), cudaMemcpyDeviceToHost, c.s_d2h));
         const u64 hi = std::min<u64>(cur, cap_ids);
@@ -1043,7 +966,7 @@ static int32_t match_host_impl(gm_engine* e, const char* blob, const uint32_t* o
         }
     }
     CUDA_TRY(cudaStreamSynchronize(c.s_d2h));
-    const u64 total = c.h_cur[nchunks - 1];
+    const u64 total = c.h_cur.as<unsigned long long>()[nchunks - 1];
     if (needed) *needed = total;
     if (total > 0xFFFFFFFFull) { g_err = "batch produces >= 2^32 output elements: split it"; return GM_ERR_TOO_LARGE; }
     if (total > cap_ids) { g_err = "output buffer too small"; return GM_ERR_CAPACITY; }
@@ -1147,10 +1070,9 @@ int32_t gm_retain_match_batch_device(gm_engine* e, const void* d_blob, uint64_t 
     if (e->flags & GM_FLAG_HOST_ONLY) { g_err = "host-only engine cannot match: there is no CPU fallback"; return GM_ERR_NO_DEVICE; }
     CUDA_TRY(cudaSetDevice(e->device));
     std::lock_guard<std::mutex> gr(e->mu_ret);      // the retained lookup's scratch is engine-wide: one lookup at a time
-    { int st = auto_flush(e, true); if (st != GM_OK) return st; }
+    GM_TRY(auto_flush(e, true));
     u64 total = 0;
-    int st = e->run_retain(d_blob, blob_bytes, d_offs, n, d_spans, d_ids, std::min<u64>(cap_ids, 0xFFFFFFFFull), d_status, static_cast<cudaStream_t>(stream), &total);
-    if (st != GM_OK) return st;
+    GM_TRY(e->run_retain(d_blob, blob_bytes, d_offs, n, d_spans, d_ids, std::min<u64>(cap_ids, 0xFFFFFFFFull), d_status, static_cast<cudaStream_t>(stream), &total));
     if (needed) *needed = total;
     if (total > 0xFFFFFFFFull) { g_err = "batch produces >= 2^32 ids: split it"; return GM_ERR_TOO_LARGE; }
     if (total > cap_ids) { g_err = "out_ids too small"; return GM_ERR_CAPACITY; }
@@ -1166,15 +1088,15 @@ int32_t gm_retain_match_batch(gm_engine* e, const char* blob, const uint32_t* of
     if (e->flags & GM_FLAG_HOST_ONLY) { g_err = "host-only engine cannot match: there is no CPU fallback"; return GM_ERR_NO_DEVICE; }
     CUDA_TRY(cudaSetDevice(e->device));
     std::lock_guard<std::mutex> gr(e->mu_ret);
-    { int st = auto_flush(e, true); if (st != GM_OK) return st; }
+    GM_TRY(auto_flush(e, true));
     if (e->knobs.small_graphs && !e->knobs.retain_stats) {      // (the per-round diagnostics come from the pipelined path)
         int st = small_graph_retain(e, blob, offsets, n, out_spans, out_ids, cap_ids, needed, status);
         if (st != GM_SMALL_NOT_APPLICABLE) return st;
     }
     const u64 blob_bytes = offsets[n];
-    MatchCtx& c = e->devctx;                          // staging of the retained host call (guarded by mu_ret)
+    MatchCtx& c = e->devctx;      // devctx's staging buffers serve only this call (the device entry points stage nothing; mu_ret guards them)
     cudaStream_t s = c.sc;
-    DevBuf &rb = e->d_rstage[0], &ro = e->d_rstage[1], &rs = e->d_rstage[2], &rt = e->d_rstage[3], &ri = e->d_rstage[4];
+    DevBuf &rb = c.d_blob, &ro = c.d_offs, &rs = c.d_spans, &rt = c.d_status, &ri = c.d_ids;
     CUDA_TRY(rb.ensure(blob_bytes + 16));
     CUDA_TRY(ro.ensure((n + 1) * sizeof(u32)));
     CUDA_TRY(rs.ensure(n * sizeof(gm_span)));
@@ -1360,21 +1282,19 @@ int32_t gm_comm_init(gm_engine* e, const uint8_t* id128, uint32_t rank, uint32_t
     NcclApi& nc = NcclApi::get();
     if (!nc.ok()) { g_err = nc.error; return GM_ERR_COMM; }
     CUDA_TRY(cudaSetDevice(e->device));
-    if (e->comm) { nc.CommDestroy(e->comm); e->comm = nullptr; }
     ncclUniqueId id;
     std::memcpy(id.internal, id128, GM_COMM_ID_BYTES);
-    NCCL_TRY(nc.CommInitRank(&e->comm, static_cast<int>(world), id, static_cast<int>(rank)));
+    NCCL_TRY(nc.CommInitRank(e->comm.put(), static_cast<int>(world), id, static_cast<int>(rank)));
     e->comm_rank = rank; e->comm_world = world;
     CUDA_TRY(e->d_comm.ensure((2 + 2 * static_cast<size_t>(world)) * sizeof(unsigned long long) + (static_cast<size_t>(world) + 2) * sizeof(u32)));
-    if (e->h_comm) { cudaFreeHost(e->h_comm); e->h_comm = nullptr; }
-    CUDA_TRY(cudaMallocHost(&e->h_comm, (2 * static_cast<size_t>(world) + 64) * sizeof(unsigned long long)));
+    CUDA_TRY(e->h_comm.ensure((2 * static_cast<size_t>(world) + 64) * sizeof(unsigned long long)));
     return GM_OK;
 }
 
 int32_t gm_comm_destroy(gm_engine* e) {
     if (!e) return GM_ERR_INVALID_ARG;
     std::lock_guard<std::mutex> g(e->mu_dev);
-    if (e->comm) { cudaSetDevice(e->device); NcclApi::get().CommDestroy(e->comm); e->comm = nullptr; }
+    if (e->comm) { cudaSetDevice(e->device); e->comm.reset(); }
     e->comm_world = 1; e->comm_rank = 0;
     return GM_OK;
 }
@@ -1420,10 +1340,11 @@ int32_t gm_allgatherv_device(gm_engine* e, const uint32_t* d_index, const gm_spa
     // 1. sizes: (k, m) of every rank.  m lives on the device (the match kernels' cursor): no host hop before the exchange.
     k_comm_sizes<<<1, 1, 0, s>>>(d_send, k, reinterpret_cast<const unsigned long long*>(d_m));
     NCCL_TRY(nc.AllGather(d_send, d_all, 2, ncclUint64, e->comm, s));
-    CUDA_TRY(cudaMemcpyAsync(e->h_comm, d_all, 2 * static_cast<size_t>(W) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(e->h_comm.p, d_all, 2 * static_cast<size_t>(W) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));      // NCCL needs the counts on the host: the one host synchronisation of the collective
     u64 K = 0, M = 0;
-    for (u32 r = 0; r < W; ++r) { sizes[2 * r] = e->h_comm[2 * r]; sizes[2 * r + 1] = e->h_comm[2 * r + 1]; K += sizes[2 * r]; M += sizes[2 * r + 1]; }
+    const unsigned long long* hc = e->h_comm.as<unsigned long long>();
+    for (u32 r = 0; r < W; ++r) { sizes[2 * r] = hc[2 * r]; sizes[2 * r + 1] = hc[2 * r + 1]; K += sizes[2 * r]; M += sizes[2 * r + 1]; }
     if (M > 0xFFFFFFFFull) { g_err = "gathered match lists exceed 2^32 ids: split the batch"; return GM_ERR_TOO_LARGE; }
     if (K > cap_topics || M > cap_ids) { g_err = "gm_allgatherv_device: output too small (sizes[] holds what every rank contributes)"; return GM_ERR_CAPACITY; }
     // 2. one grouped launch, straight out of the buffers the match kernels wrote.  Default: point-to-point (every rank sends
@@ -1534,14 +1455,13 @@ int32_t gm_match_gather_device(gm_engine* e, const void* d_blob, uint64_t blob_b
     if (!G.connected) { g_err = "gm_match_gather_device: gm_gather_create + gm_gather_connect first"; return GM_ERR_INVALID_ARG; }
     if (n > G.slab_topics) { g_err = "gm_match_gather_device: more rows than this rank's slab holds"; return GM_ERR_CAPACITY; }
     CUDA_TRY(cudaSetDevice(e->device));
-    { int st = auto_flush(e); if (st != GM_OK) return st; }
+    GM_TRY(auto_flush(e));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     std::lock_guard<std::mutex> gd(e->mu_dev);
     const GatherTarget target{&G, G.peer, G.rank, e->knobs.gather_direct};
     gm_engine::MatchCall a;
     a.blob = d_blob; a.blob_bytes = blob_bytes; a.offs = d_offsets; a.sel = d_sel; a.n = n; a.cap = G.slab_ids; a.status = d_status; a.gather = &target;
-    int st = e->enqueue_match(e->devctx, a, s);
-    if (st != GM_OK) return st;
+    GM_TRY(e->enqueue_match(e->devctx, a, s));
     // contribution (rows, ids) into every rank's counts + the epoch barrier: when it has passed on a rank, all ranks' data is there
     G.epoch++;
     const unsigned long long* d_m = n ? &e->devctx.d_ctrl.as<Ctrl>()->cursor : nullptr;
@@ -1586,9 +1506,7 @@ int32_t gm_gather_destroy(gm_engine* e) {
     if (!G.block) return GM_OK;
     cudaSetDevice(e->device);
     cudaDeviceSynchronize();
-    for (u32 w = 0; w < G.world; ++w) if (w != G.rank && G.peer[w]) cudaIpcCloseMemHandle(G.peer[w]);
-    cudaFree(G.block);
-    G = gm_engine::Gather{};
+    G.close();
     return GM_OK;
 }
 
@@ -1690,7 +1608,7 @@ int32_t gm_kernel_ms_ring(gm_engine* e, float* out_ms, uint32_t max_calls, uint3
     const u64 have = std::min<u64>(e->ring_n, gm_engine::RING);
     const u64 take = std::min<u64>(have, max_calls);
     for (u64 k = 0; k < take; ++k) {                       // oldest first
-        cudaEvent_t* ev = e->ev_ring[(e->ring_n - take + k) % gm_engine::RING];
+        const Event* ev = e->ev_ring[(e->ring_n - take + k) % gm_engine::RING];
         CUDA_TRY(cudaEventSynchronize(ev[3]));
         for (int j = 0; j < 3; ++j) CUDA_TRY(cudaEventElapsedTime(&out_ms[3 * k + j], ev[j], ev[j + 1]));
     }

@@ -13,24 +13,6 @@ std::string ckey(uint64_t node, const std::string& client) { std::string k = std
 std::string ikey(uint64_t node, const std::string& client, uint64_t tag) { std::string k = ckey(node, client); k.push_back('\0'); k += std::to_string(tag); return k; }
 }  // namespace
 
-#define R_TRY0(expr) do { int32_t _rc = (expr); if (_rc != GM_OK) return _rc; } while (0)
-
-GpuRouter::~GpuRouter() {
-    for (Dev* d : {&d_rels_, &d_blob_, &d_offs_, &d_spans_, &d_status_, &d_ids_, &d_needed_, &d_pubs_, &d_ospans_, &d_orels_, &d_subs_, &d_ghdr_, &d_gmem_, &d_online_})
-        if (d->p) cudaFree(d->p);
-    if (stream_) cudaStreamDestroy(static_cast<cudaStream_t>(stream_));
-}
-
-int32_t GpuRouter::ensure(Dev& d, size_t bytes) {
-    if (bytes <= d.cap) return GM_OK;
-    size_t ncap = std::max(bytes, d.cap + d.cap / 2 + 4096);
-    void* np = nullptr;
-    if (cudaMalloc(&np, ncap) != cudaSuccess) return GM_ERR_CUDA;
-    if (d.p) { cudaMemcpy(np, d.p, d.cap, cudaMemcpyDeviceToDevice); cudaFree(d.p); }
-    d.p = np; d.cap = ncap;
-    return GM_OK;
-}
-
 // client keys number the (node id, client id) pairs in order of first appearance; a new key starts online
 uint32_t GpuRouter::client_key(uint64_t node_id, const std::string& client) {
     const uint32_t k = intern(client_key_, ckey(node_id, client));
@@ -221,7 +203,7 @@ int32_t GpuRouter::matched_filters_batch(const char* blob, const uint32_t* offs,
         break;
     }
     gm_values vv{};
-    R_TRY0(gm_values_view(e_, &vv));
+    GM_TRY(gm_values_view(e_, &vv));
     for (uint64_t i = 0; i < n; ++i) {
         const size_t begin = filters.size();
         if (status[i] == 0) {
@@ -276,24 +258,21 @@ int32_t GpuRouter::host_dedup_topic(const gm_sub_relation* in, uint32_t cnt, boo
     return GM_OK;
 }
 
-#define R_CUDA(expr) do { cudaError_t _ce = (expr); if (_ce != cudaSuccess) return (_ce == cudaErrorNoDevice || _ce == cudaErrorInsufficientDriver) ? GM_ERR_NO_DEVICE : GM_ERR_CUDA; } while (0)
-#define R_TRY(expr) do { int32_t _rc = (expr); if (_rc != GM_OK) return _rc; } while (0)
-
-// the group header, member pool and online bitmap: what changed since the last choosing call
-int32_t GpuRouter::ship_groups(void* stream) {
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    auto ship = [&](Dev& d, const void* host, size_t elem, size_t count, Dirty& dirty) -> int32_t {
-        R_TRY(ensure(d, std::max<size_t>(count, 256) * elem));
+// the group header, member pool and online bitmap: what changed since the last choosing call (a table that grows keeps its
+// contents: only the dirty range is shipped)
+int32_t GpuRouter::ship_groups(cudaStream_t s) {
+    auto ship = [&](DevBuf& d, const void* host, size_t elem, size_t count, Dirty& dirty) -> int32_t {
+        CUDA_TRY(d.ensure(std::max<size_t>(count, 256) * elem, true, s));
         if (dirty.any()) {
             const size_t lo = dirty.lo, hi = std::min<size_t>(dirty.hi, count);
-            if (hi > lo) R_CUDA(cudaMemcpyAsync(static_cast<char*>(d.p) + lo * elem, static_cast<const char*>(host) + lo * elem, (hi - lo) * elem, cudaMemcpyHostToDevice, s));
+            if (hi > lo) CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(d.p) + lo * elem, static_cast<const char*>(host) + lo * elem, (hi - lo) * elem, cudaMemcpyHostToDevice, s));
             dirty = Dirty{};
         }
         return GM_OK;
     };
-    R_TRY(ship(d_ghdr_, grp_hdr_.data(), sizeof(gm_span), grp_hdr_.size(), hdr_dirty_));
-    R_TRY(ship(d_gmem_, member_pool_.data(), 4, member_pool_.size(), pool_dirty_));
-    R_TRY(ship(d_online_, online_words_.data(), 4, online_words_.size(), online_dirty_));
+    GM_TRY(ship(d_ghdr_, grp_hdr_.data(), sizeof(gm_span), grp_hdr_.size(), hdr_dirty_));
+    GM_TRY(ship(d_gmem_, member_pool_.data(), 4, member_pool_.size(), pool_dirty_));
+    GM_TRY(ship(d_online_, online_words_.data(), 4, online_words_.size(), online_dirty_));
     return GM_OK;
 }
 
@@ -308,51 +287,51 @@ int32_t GpuRouter::matches_batch(const gm_id* publishers, const char* blob, cons
     if (n == 0) return GM_OK;
     using Clk = std::chrono::steady_clock;
     const auto t0 = Clk::now();
-    if (!stream_) { cudaStream_t s; R_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); stream_ = s; }
-    cudaStream_t s = static_cast<cudaStream_t>(stream_);
+    if (!stream_) CUDA_TRY(cudaStreamCreateWithFlags(stream_.put(), cudaStreamNonBlocking));
+    const cudaStream_t s = stream_;
     if (share_seed) {
         // a group's representative must be in the device trie, also on an engine that only flushes when told to
-        if (groups_changed_) { R_TRY(gm_flush(e_)); groups_changed_ = false; unflushed_removes_ = false; }
-        R_TRY(ship_groups(s));
+        if (groups_changed_) { GM_TRY(gm_flush(e_)); groups_changed_ = false; unflushed_removes_ = false; }
+        GM_TRY(ship_groups(s));
     }
     // ---- the relation table: ship what changed since the last call
     if (rel_dirty_hi_ > rel_dirty_lo_) {
-        R_TRY(ensure(d_rels_, std::max<size_t>(rel_host_.size(), 1024) * sizeof(gm_rel)));
-        R_CUDA(cudaMemcpyAsync(static_cast<gm_rel*>(d_rels_.p) + rel_dirty_lo_, rel_host_.data() + rel_dirty_lo_, (rel_dirty_hi_ - rel_dirty_lo_) * sizeof(gm_rel), cudaMemcpyHostToDevice, s));
+        CUDA_TRY(d_rels_.ensure(std::max<size_t>(rel_host_.size(), 1024) * sizeof(gm_rel), true, s));
+        CUDA_TRY(cudaMemcpyAsync(static_cast<gm_rel*>(d_rels_.p) + rel_dirty_lo_, rel_host_.data() + rel_dirty_lo_, (rel_dirty_hi_ - rel_dirty_lo_) * sizeof(gm_rel), cudaMemcpyHostToDevice, s));
         rel_dirty_lo_ = 0xFFFFFFFFu; rel_dirty_hi_ = 0;
     }
     // ---- topics and publishers to the device, match (ids = relation handles stay in HBM)
     const uint64_t blob_bytes = offs[n];
-    R_TRY(ensure(d_blob_, blob_bytes + 16)); R_TRY(ensure(d_offs_, (n + 1) * 4)); R_TRY(ensure(d_spans_, n * 8)); R_TRY(ensure(d_status_, n * 4));
-    R_TRY(ensure(d_needed_, 4 * 8)); R_TRY(ensure(d_ospans_, n * 8));
-    if (blob_bytes) R_CUDA(cudaMemcpyAsync(d_blob_.p, blob, blob_bytes, cudaMemcpyHostToDevice, s));
-    R_CUDA(cudaMemcpyAsync(d_offs_.p, offs, (n + 1) * 4, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(d_blob_.ensure(blob_bytes + 16)); CUDA_TRY(d_offs_.ensure((n + 1) * 4)); CUDA_TRY(d_spans_.ensure(n * 8)); CUDA_TRY(d_status_.ensure(n * 4));
+    CUDA_TRY(d_needed_.ensure(4 * 8)); CUDA_TRY(d_ospans_.ensure(n * 8));
+    if (blob_bytes) CUDA_TRY(cudaMemcpyAsync(d_blob_.p, blob, blob_bytes, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_offs_.p, offs, (n + 1) * 4, cudaMemcpyHostToDevice, s));
     if (publishers) {
         pubs_.resize(n);
         for (uint64_t i = 0; i < n; ++i) {
             auto it = id_idx_.find(ikey(publishers[i].node_id, publishers[i].client_id ? std::string(publishers[i].client_id, publishers[i].client_len) : std::string(), publishers[i].tag));
             pubs_[i] = it == id_idx_.end() ? 0xFFFFFFFFu : it->second;       // an Id no subscriber holds cannot equal any relation's Id
         }
-        R_TRY(ensure(d_pubs_, n * 4));
-        R_CUDA(cudaMemcpyAsync(d_pubs_.p, pubs_.data(), n * 4, cudaMemcpyHostToDevice, s));
+        CUDA_TRY(d_pubs_.ensure(n * 4));
+        CUDA_TRY(cudaMemcpyAsync(d_pubs_.p, pubs_.data(), n * 4, cudaMemcpyHostToDevice, s));
     }
-    if (d_ids_.cap < 4096) R_TRY(ensure(d_ids_, std::max<size_t>(4096, 32 * n) * 4));
+    if (d_ids_.cap < 4096) CUDA_TRY(d_ids_.ensure(std::max<size_t>(4096, 32 * n) * 4));
     uint64_t need[4] = {0, 0, 0, 0};
     for (;;) {
         gm_match_args a{};
         a.struct_size = sizeof(a); a.d_blob = d_blob_.p; a.blob_bytes = blob_bytes; a.d_offsets = static_cast<const uint32_t*>(d_offs_.p); a.n_entries = n; a.n = n;
         a.d_spans = static_cast<gm_span*>(d_spans_.p); a.d_out = d_ids_.p; a.cap = d_ids_.cap / 4; a.d_needed = static_cast<uint64_t*>(d_needed_.p) + 3;
         a.d_status = static_cast<int32_t*>(d_status_.p); a.stream = s;
-        R_TRY(gm_match_batch_device_ex(e_, &a));
-        R_CUDA(cudaMemcpyAsync(&need[3], static_cast<uint64_t*>(d_needed_.p) + 3, 8, cudaMemcpyDeviceToHost, s));
-        R_CUDA(cudaStreamSynchronize(s));
+        GM_TRY(gm_match_batch_device_ex(e_, &a));
+        CUDA_TRY(cudaMemcpyAsync(&need[3], static_cast<uint64_t*>(d_needed_.p) + 3, 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
         if (need[3] > 0xFFFFFFFFull) return GM_ERR_TOO_LARGE;
         if (need[3] * 4 <= d_ids_.cap) break;
-        R_TRY(ensure(d_ids_, (need[3] + 1024) * 4));
+        CUDA_TRY(d_ids_.ensure((need[3] + 1024) * 4));
     }
     // ---- relation expansion on the device: at most one record and one sub id per matched id
-    R_TRY(ensure(d_orels_, std::max<uint64_t>(need[3], 1) * sizeof(gm_sub_relation)));
-    R_TRY(ensure(d_subs_, std::max<uint64_t>(need[3], 1) * 4));
+    CUDA_TRY(d_orels_.ensure(std::max<uint64_t>(need[3], 1) * sizeof(gm_sub_relation)));
+    CUDA_TRY(d_subs_.ensure(std::max<uint64_t>(need[3], 1) * 4));
     gm_rel_out o{};
     o.d_spans = static_cast<gm_span*>(d_ospans_.p); o.d_rels = static_cast<gm_sub_relation*>(d_orels_.p); o.cap_rels = d_orels_.cap / sizeof(gm_sub_relation);
     o.d_sub_ids = static_cast<uint32_t*>(d_subs_.p); o.cap_sub_ids = d_subs_.cap / 4;
@@ -361,24 +340,24 @@ int32_t GpuRouter::matches_batch(const gm_id* publishers, const char* blob, cons
         gm_rel_groups gr{};
         gr.d_groups = static_cast<const gm_span*>(d_ghdr_.p); gr.n_groups = static_cast<uint32_t>(grp_hdr_.size()); gr.d_members = static_cast<const uint32_t*>(d_gmem_.p);
         gr.d_online = static_cast<const uint32_t*>(d_online_.p); gr.n_online_bits = static_cast<uint32_t>(client_key_.size()); gr.seed = *share_seed;
-        R_TRY(gm_relations_choose_device(e_, static_cast<const gm_span*>(d_spans_.p), static_cast<const uint32_t*>(d_ids_.p), n, publishers ? static_cast<const uint32_t*>(d_pubs_.p) : nullptr,
+        GM_TRY(gm_relations_choose_device(e_, static_cast<const gm_span*>(d_spans_.p), static_cast<const uint32_t*>(d_ids_.p), n, publishers ? static_cast<const uint32_t*>(d_pubs_.p) : nullptr,
                                          static_cast<const gm_rel*>(d_rels_.p), rel_host_.size(), &gr, &o, s));
     } else
-        R_TRY(gm_relations_expand_device(e_, static_cast<const gm_span*>(d_spans_.p), static_cast<const uint32_t*>(d_ids_.p), n, publishers ? static_cast<const uint32_t*>(d_pubs_.p) : nullptr,
+        GM_TRY(gm_relations_expand_device(e_, static_cast<const gm_span*>(d_spans_.p), static_cast<const uint32_t*>(d_ids_.p), n, publishers ? static_cast<const uint32_t*>(d_pubs_.p) : nullptr,
                                          static_cast<const gm_rel*>(d_rels_.p), rel_host_.size(), &o, s));
-    R_CUDA(cudaMemcpyAsync(need, d_needed_.p, 2 * 8, cudaMemcpyDeviceToHost, s));
-    R_CUDA(cudaMemcpyAsync(status, d_status_.p, n * 4, cudaMemcpyDeviceToHost, s));
-    R_CUDA(cudaMemcpyAsync(out_spans, d_ospans_.p, n * 8, cudaMemcpyDeviceToHost, s));
-    R_CUDA(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaMemcpyAsync(need, d_needed_.p, 2 * 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(status, d_status_.p, n * 4, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(out_spans, d_ospans_.p, n * 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
     bool flagged = false;
     for (uint64_t i = 0; i < n && !flagged; ++i) flagged = status[i] == 1;
     if (!flagged) {      // the common case: the device's records ARE the result
         if (needed_rels) *needed_rels = need[0];
         if (needed_sub_ids) *needed_sub_ids = need[1];
         if (need[0] > cap_rels || need[1] > cap_sub_ids) return GM_ERR_CAPACITY;
-        if (need[0]) R_CUDA(cudaMemcpyAsync(out_rels, d_orels_.p, need[0] * sizeof(gm_sub_relation), cudaMemcpyDeviceToHost, s));
-        if (need[1]) R_CUDA(cudaMemcpyAsync(out_sub_ids, d_subs_.p, need[1] * 4, cudaMemcpyDeviceToHost, s));
-        R_CUDA(cudaStreamSynchronize(s));
+        if (need[0]) CUDA_TRY(cudaMemcpyAsync(out_rels, d_orels_.p, need[0] * sizeof(gm_sub_relation), cudaMemcpyDeviceToHost, s));
+        if (need[1]) CUDA_TRY(cudaMemcpyAsync(out_sub_ids, d_subs_.p, need[1] * 4, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
         last_device_ms = std::chrono::duration<double, std::milli>(Clk::now() - t0).count();
         last_host_ms = 0;
         return GM_OK;
@@ -387,14 +366,14 @@ int32_t GpuRouter::matches_batch(const gm_id* publishers, const char* blob, cons
     const auto t1 = Clk::now();
     std::vector<gm_sub_relation> dev(need[0]), rels;
     std::vector<uint32_t> dsub(need[1]), sub_ids;
-    if (need[0]) R_CUDA(cudaMemcpyAsync(dev.data(), d_orels_.p, need[0] * sizeof(gm_sub_relation), cudaMemcpyDeviceToHost, s));
-    if (need[1]) R_CUDA(cudaMemcpyAsync(dsub.data(), d_subs_.p, need[1] * 4, cudaMemcpyDeviceToHost, s));
-    R_CUDA(cudaStreamSynchronize(s));
+    if (need[0]) CUDA_TRY(cudaMemcpyAsync(dev.data(), d_orels_.p, need[0] * sizeof(gm_sub_relation), cudaMemcpyDeviceToHost, s));
+    if (need[1]) CUDA_TRY(cudaMemcpyAsync(dsub.data(), d_subs_.p, need[1] * 4, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
     rels.reserve(need[0]);
     for (uint64_t i = 0; i < n; ++i) {
         const size_t begin = rels.size();
         const uint32_t off = out_spans[i].off, cnt = out_spans[i].cnt;
-        if (status[i] == 1) { status[i] = 0; R_TRY(host_dedup_topic(dev.data() + off, cnt, share_seed != nullptr, rels, sub_ids)); }
+        if (status[i] == 1) { status[i] = 0; GM_TRY(host_dedup_topic(dev.data() + off, cnt, share_seed != nullptr, rels, sub_ids)); }
         else if (status[i] == 0)
             for (uint32_t k = 0; k < cnt; ++k) {
                 gm_sub_relation sr = dev[off + k];

@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/gpumqtt.h"
+#include "cuda_owned.h"
 
 namespace gm {
 
@@ -35,7 +36,6 @@ class GpuRouter {
     struct Opts { uint8_t qos = 0, is_v5 = 0, no_local = 0; uint32_t sub_id = 0; std::string group; };                          // types.rs:565-718
 
     explicit GpuRouter(gm_engine* e) : e_(e) {}
-    ~GpuRouter();
     // timing of the last matches_batch call (milliseconds): device (H2D + match + relation kernel + D2H), host assembly
     double last_device_ms = 0, last_host_ms = 0;
 
@@ -67,16 +67,14 @@ class GpuRouter {
     std::vector<uint32_t> free_handles_;
     bool unflushed_removes_ = false;
     int64_t topics_ = 0, routes_ = 0;
-    std::vector<gm_span> tmp_spans_;
-    std::vector<uint32_t> tmp_ids_;
     // ---- device side of the relation expansion ----
     std::vector<gm_rel> rel_host_;                                     // handle -> record, mirrored in HBM
     uint32_t rel_dirty_lo_ = 0xFFFFFFFFu, rel_dirty_hi_ = 0;           // handles changed since the last upload
     std::unordered_map<std::string, uint32_t> client_key_, id_idx_;    // "node\0client" -> key, "node\0client\0tag" -> idx
-    struct Dev { void* p = nullptr; size_t cap = 0; };
-    Dev d_rels_, d_blob_, d_offs_, d_spans_, d_status_, d_ids_, d_needed_, d_pubs_, d_ospans_, d_orels_, d_subs_;
+    DevBuf d_rels_;                                                    // shipped by dirty range: grows with its contents kept
+    DevBuf d_blob_, d_offs_, d_spans_, d_status_, d_ids_, d_needed_, d_pubs_, d_ospans_, d_orels_, d_subs_;   // one call's scratch
     std::vector<uint32_t> pubs_;
-    void* stream_ = nullptr;
+    Stream stream_;                                                    // created by the first matches_batch
     // ---- shared groups in device layout (k_relations<true>): group id -> a block of live member handles with spare room in one
     //      pool; a block that fills up moves to the pool's end, and the pool is re-packed once the abandoned blocks pass half of it.
     //      The header, the pool and the online bitmap are shipped by dirty range, like rel_host_.
@@ -90,15 +88,14 @@ class GpuRouter {
     Dirty hdr_dirty_, pool_dirty_, online_dirty_;                      // online_dirty_ counts words
     bool groups_changed_ = false;                                      // membership changed since the router's last gm_flush
     std::vector<uint32_t> online_words_;                               // bit per client_key, 1 = online
-    Dev d_ghdr_, d_gmem_, d_online_;
-    int32_t ensure(Dev& d, size_t bytes);
+    DevBuf d_ghdr_, d_gmem_, d_online_;
     uint32_t intern(std::unordered_map<std::string, uint32_t>& m, const std::string& k) { return m.emplace(k, static_cast<uint32_t>(m.size())).first->second; }
     uint32_t client_key(uint64_t node_id, const std::string& client);
     void set_rel(uint32_t handle, const Rel& r);
     void member_add(uint32_t group, uint32_t handle);
     void member_remove(uint32_t handle);
     void repack_groups();
-    int32_t ship_groups(void* stream);
+    int32_t ship_groups(cudaStream_t s);
     int32_t host_dedup_topic(const gm_sub_relation* in, uint32_t cnt, bool chosen, std::vector<gm_sub_relation>& rels, std::vector<uint32_t>& sub_ids);
 };
 
