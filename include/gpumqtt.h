@@ -203,6 +203,37 @@ int32_t gm_retain_match_batch_device(gm_engine* e, const void* d_filters_blob, u
                                      const uint32_t* d_filter_offsets, uint64_t n, gm_span* d_out_spans,
                                      uint32_t* d_out_ids, uint64_t cap_ids, uint64_t* needed, int32_t* d_status, void* stream);
 
+/* ---- expiry of retained messages: RetainTree<TimedValue<Retain>> (rmqtt/src/retain.rs:100-170, types.rs:2275-2296).
+ * A deadline is a uint64_t in milliseconds since the Unix epoch (rmqtt's timestamp_millis); 0 means no deadline.  A value is
+ * expired iff now >= deadline (TimedValue::is_expired).  The message store tests `expiry_time_at < now`
+ * (types.rs:1883-1885): its callers pass expiry_time_at + 1.
+ *   - A deadline belongs to a handle.  A handle that carries a deadline is stored under one topic only: storing it under a
+ *     second topic, through gm_retain_set or gm_retain_set_ttl, returns GM_ERR_INVALID_ARG and changes nothing.  (The lookup
+ *     checks deadlines by handle, so a handle stored without one under other topics must not be given one.)
+ *   - Setting a handle without a deadline (gm_retain_set, or deadline_ms = 0) clears its deadline (set_with_timeout(.., None),
+ *     retain.rs:131-149).  A value that is replaced or removed loses its deadline.
+ *   - Handles with a deadline are below GM_RETAIN_TTL_MAX_HANDLE: the device keeps one 8-byte word per handle up to the
+ *     largest of them.  Values set through the calls without a deadline never expire.
+ * gm_retain_match_batch, gm_retain_match_batch_device and the retained batcher are gm_retain_match_batch_at at the wall
+ * clock, read once per lookup.  An engine that holds no deadline runs the lookup exactly as without this section.          */
+#define GM_RETAIN_TTL_MAX_HANDLE (1u << 28)
+int32_t gm_retain_set_ttl(gm_engine* e, const char* topic, uint32_t len, uint32_t value, uint64_t deadline_ms,
+                          int32_t* had_old, uint32_t* old_value);
+/* gm_retain_bulk_load with a deadline per entry (0: none), as n gm_retain_set_ttl calls in order and on the same parallel build
+ * into an empty tree.  A batch that would store a handle with a deadline under a second topic changes nothing
+ * (GM_ERR_INVALID_ARG).                                                                                                      */
+int32_t gm_retain_bulk_load_ttl(gm_engine* e, const char* blob, const uint32_t* offsets /* n+1 */, const uint32_t* values,
+                                const uint64_t* deadlines_ms, uint64_t n, uint64_t* n_set);
+/* RetainStorage::get at `now_ms`: gm_retain_match_batch without the expired handles.  `needed` and the spans count live
+ * handles only; same capacity / status protocol.                                                                          */
+int32_t gm_retain_match_batch_at(gm_engine* e, uint64_t now_ms, const char* filters_blob, const uint32_t* filter_offsets, uint64_t n,
+                                 gm_span* out_spans, uint32_t* out_ids, uint64_t cap_ids, uint64_t* needed, int32_t* status);
+/* remove_expired_messages (retain.rs:118-128): removes at most `cap` topics whose handle expired at now_ms, earliest deadline
+ * first, under one lock acquisition; they ship with the next flush like any removal.  out_values[0 .. *n_removed) receives
+ * their handles, so that the caller can drop the payloads.  Loop while *n_removed == cap.  The cost grows with the number
+ * removed (a deadline-ordered queue), not with the size of the tree.                                                      */
+int32_t gm_retain_remove_expired(gm_engine* e, uint64_t now_ms, uint32_t* out_values, uint64_t cap, uint64_t* n_removed);
+
 /* ---- GpuRouter: DefaultRouter's Router-level semantics above the engine (rmqtt/src/router.rs:109-115, 162-248,
  *      417-479; rmqtt/src/types.rs:470-508).  This is what a Rust `GpuRouter` keeps on the host (INTEGRATION.md);
  *      it is provided in C++ because the reference toolchain is absent from the build image.                  */

@@ -107,6 +107,16 @@ extern "C" {
     pub fn gm_match_batch_trees(e: *mut gm_engine, topics_blob: *const u8, topic_offsets: *const u32, trees: *const u32, n: u64,
                                 out_spans: *mut gm_span, out_ids: *mut u32, cap_ids: u64, needed: *mut u64, status: *mut i32) -> i32;
     pub fn gm_retain_remove_batch(e: *mut gm_engine, blob: *const u8, offsets: *const u32, n: u64, old_values: *mut u32, n_removed: *mut u64) -> i32;
+    /// Expiry (RetainTree<TimedValue<Retain>>): deadlines in ms since the Unix epoch, 0 = none; expired iff now >= deadline.
+    /// A handle with a deadline is stored under one topic only (a second one: GM_ERR_INVALID_ARG, nothing changed).
+    pub fn gm_retain_set_ttl(e: *mut gm_engine, topic: *const u8, len: u32, value: u32, deadline_ms: u64, had_old: *mut i32, old_value: *mut u32) -> i32;
+    pub fn gm_retain_bulk_load_ttl(e: *mut gm_engine, blob: *const u8, offsets: *const u32, values: *const u32, deadlines_ms: *const u64, n: u64,
+                                   n_set: *mut u64) -> i32;
+    /// gm_retain_match_batch at `now_ms` (gm_retain_match_batch itself uses the wall clock).
+    pub fn gm_retain_match_batch_at(e: *mut gm_engine, now_ms: u64, filters_blob: *const u8, filter_offsets: *const u32, n: u64, out_spans: *mut gm_span,
+                                    out_ids: *mut u32, cap_ids: u64, needed: *mut u64, status: *mut i32) -> i32;
+    /// remove_expired_messages: up to `cap` expired topics in one lock acquisition; their handles go to out_values.
+    pub fn gm_retain_remove_expired(e: *mut gm_engine, now_ms: u64, out_values: *mut u32, cap: u64, n_removed: *mut u64) -> i32;
 }
 
 // ---- the rest of include/gpumqtt.h: device-buffer entry points, router level, relation expansion, multi-GPU, probes ----

@@ -11,13 +11,14 @@
 #![deny(unsafe_code)] // all `unsafe` lives in `engine` below, a private module with a safe surface
 use std::sync::atomic::{AtomicU32, Ordering};
 use std::sync::Arc;
-use std::time::{Duration, Instant};
+use std::time::Duration;
 
 use async_trait::async_trait;
 use dashmap::DashMap;
 use itertools::Itertools;
 use rmqtt::{
     context::ServerContext,
+    utils::timestamp_millis,   // ms since the Unix epoch (rmqtt-utils/src/lib.rs:504): the unit of the engine's deadlines
     macros::Plugin,
     plugin::{PackageInfo, Plugin},
     register,
@@ -95,7 +96,23 @@ mod engine {
             if rc != sys::GM_OK { return Err(self.err("gm_retain_remove", rc)) }
             Ok((had != 0).then_some(old))
         }
-        /// The expiry sweep (rmqtt-retainer/src/lib.rs:112-124 -> RetainTree::retain, retain.rs:261-288) as ONE call.
+        /// set_with_timeout: `deadline_ms` in ms since the Unix epoch (0 = none); the lookups drop the handle from then on.
+        pub fn retain_set_ttl(&self, topic: &str, value: u32, deadline_ms: u64) -> anyhow::Result<Option<u32>> {
+            let (mut had, mut old) = (0, 0);
+            let rc = unsafe { sys::gm_retain_set_ttl(self.0, topic.as_ptr(), topic.len() as u32, value, deadline_ms, &mut had, &mut old) };
+            if rc != sys::GM_OK { return Err(self.err("gm_retain_set_ttl", rc)) }
+            Ok((had != 0).then_some(old))
+        }
+        /// remove_expired_messages (retain.rs:118-128): up to `cap` expired topics per call; their handles come back.
+        pub fn retain_remove_expired(&self, now_ms: u64, cap: usize) -> anyhow::Result<Vec<u32>> {
+            let mut out = vec![0u32; cap];
+            let mut n = 0u64;
+            let rc = unsafe { sys::gm_retain_remove_expired(self.0, now_ms, out.as_mut_ptr(), cap as u64, &mut n) };
+            if rc != sys::GM_OK { return Err(self.err("gm_retain_remove_expired", rc)) }
+            out.truncate(n as usize);
+            Ok(out)
+        }
+        /// Removal of a list of topics as ONE call (RetainTree::retain, retain.rs:261-288).
         pub fn retain_remove_batch(&self, topics: &[&str]) -> anyhow::Result<u64> {
             let (mut blob, mut offs) = (Vec::new(), vec![0u32]);
             for t in topics { blob.extend_from_slice(t.as_bytes()); offs.push(blob.len() as u32); }
@@ -407,7 +424,8 @@ impl Router for GpuRouter {
 
 // ---- retainer -------------------------------------------------------------------------------------------------------
 /// One slot per retained topic, indexed by the handle stored in the device tree: `get` never walks a CPU `RetainTree`.
-struct Slot { topic: TopicName, retain: Retain, expiry: Option<Instant> }
+/// The engine keeps the deadlines (gm_retain_set_ttl): its lookups return live handles only.
+struct Slot { topic: TopicName, retain: Retain }
 
 #[derive(Clone)]
 pub struct GpuRetainer {
@@ -424,15 +442,17 @@ impl GpuRetainer {
         Ok(Self { engine, batcher, slots: Arc::new(DashMap::default()), next: Arc::new(AtomicU32::new(0)) })
     }
 
-    /// retain.rs:118-128 (`remove_expired_messages`): the host decides what expired, the tree forgets it in one call
+    /// retain.rs:118-128 (`remove_expired_messages`): the engine's deadline queue yields the expired topics, a batch per call
     async fn remove_expired_messages(&self) -> usize {
-        let now = Instant::now();
-        let dead: Vec<(u32, TopicName)> = self.slots.iter().filter(|e| e.expiry.map(|t| t <= now).unwrap_or(false)).map(|e| (*e.key(), e.topic.clone())).collect();
-        if dead.is_empty() { return 0 }
-        let names: Vec<&str> = dead.iter().map(|(_, t)| t.as_ref()).collect();
-        let _ = self.engine.retain_remove_batch(&names);
-        for (h, _) in &dead { self.slots.remove(h); }
-        dead.len()
+        const CAP: usize = 65_536;
+        let now = timestamp_millis() as u64;
+        let mut n = 0;
+        loop {
+            let dead = self.engine.retain_remove_expired(now, CAP).unwrap_or_default();
+            for h in &dead { self.slots.remove(h); }
+            n += dead.len();
+            if dead.len() < CAP { return n }
+        }
     }
 }
 
@@ -447,16 +467,16 @@ impl RetainStorage for GpuRetainer {
             return Ok(());
         }
         let h = self.next.fetch_add(1, Ordering::Relaxed);
-        self.slots.insert(h, Slot { topic: topic.clone(), retain, expiry: expiry_interval.map(|d| Instant::now() + d) });
-        if let Some(old) = self.engine.retain_set(topic, h)? { self.slots.remove(&old); } // Option::replace semantics
+        let deadline = expiry_interval.map(|d| timestamp_millis() as u64 + d.as_millis() as u64).unwrap_or(0);
+        self.slots.insert(h, Slot { topic: topic.clone(), retain });
+        if let Some(old) = self.engine.retain_set_ttl(topic, h, deadline)? { self.slots.remove(&old); } // Option::replace semantics
         Ok(())
     }
 
-    /// retain.rs:152-169: expired entries are dropped, the rest cloned out
+    /// retain.rs:152-169: the device already dropped the expired handles; the rest are cloned out
     async fn get(&self, topic_filter: &TopicFilter) -> Result<Vec<(TopicName, Retain)>> {
         let ids = self.batcher.submit(topic_filter.as_ref())?.await?.map_err(|st| anyhow::anyhow!("retained lookup failed ({st})"))?;
-        let now = Instant::now();
-        Ok(ids.into_iter().filter_map(|h| self.slots.get(&h).filter(|s| s.expiry.map(|t| t > now).unwrap_or(true)).map(|s| (s.topic.clone(), s.retain.clone()))).collect())
+        Ok(ids.into_iter().filter_map(|h| self.slots.get(&h).map(|s| (s.topic.clone(), s.retain.clone()))).collect())
     }
 
     async fn count(&self) -> isize { self.slots.len() as isize }

@@ -163,6 +163,10 @@ SIGNATURES = {
     "gm_retain_bulk_load": (_i32, [_vp, _vp, _vp, _vp, _u64, _P(_u64)]),
     "gm_retain_match_batch": (_i32, [_vp, _vp, _vp, _u64, _vp, _vp, _u64, _P(_u64), _vp]),
     "gm_retain_match_batch_device": (_i32, [_vp, _vp, _u64, _vp, _u64, _vp, _vp, _u64, _P(_u64), _vp, _vp]),
+    "gm_retain_set_ttl": (_i32, [_vp, _cp, _u32, _u32, _u64, _P(_i32), _P(_u32)]),
+    "gm_retain_bulk_load_ttl": (_i32, [_vp, _vp, _vp, _vp, _vp, _u64, _P(_u64)]),
+    "gm_retain_match_batch_at": (_i32, [_vp, _u64, _vp, _vp, _u64, _vp, _vp, _u64, _P(_u64), _vp]),
+    "gm_retain_remove_expired": (_i32, [_vp, _u64, _vp, _u64, _P(_u64)]),
     "gmr_create": (_i32, [_vp, _P(_vp)]),
     "gmr_destroy": (None, [_vp]),
     "gmr_add": (_i32, [_vp, _cp, _u32, _P(GmId), _P(GmSubOpts)]),

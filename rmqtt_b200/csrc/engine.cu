@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <cctype>
+#include <chrono>
 #include <cstddef>
 #include <cstdio>
 #include <cstdlib>
@@ -115,7 +116,9 @@ struct gm_engine {
     std::vector<DevBuf> retired;     // table buffers replaced by an epoch swap: freed once every match that could see them is done
     // retained tree (device copy of the flattened arrays) + scratch of the retained lookup
     DevBuf d_rnodes, d_rkids, d_redges, d_rvals;
+    DevBuf d_rdl;                    // deadline per handle (u64, ~0 = none), shipped once a handle was given one
     DevBuf d_rfront[2], d_rdescs, d_rctl, d_rq;
+    DevBuf d_rnow; PinnedBuf h_rnow; // the pipelined lookup's `now` (small graphs carry theirs in the in-block header)
     u32 r_cap_items = 1u << 22, r_cap_desc = 1u << 22;   // totals over the RQ slices of each queue
     std::unique_ptr<SmallGraph> rsmall[2];   // small retained lookups as one CUDA-graph launch (small_graph_retain; mu_ret)
     u64 launches = 0;
@@ -161,7 +164,8 @@ struct gm_engine {
     // GM_FLAG_MANUAL_FLUSH the host mirror may already have grown / re-hashed a table that the device has not seen yet.
     TrieView dev_view{};
     RetainView dev_rview{};
-    size_t up_rkids = 0, up_rvals = 0, up_redges_slots = 0;
+    u32 dev_rdl_n = 0;               // handles the shipped deadline table covers; 0: the tree held no deadline at the last flush
+    size_t up_rkids = 0, up_rvals = 0, up_redges_slots = 0, up_rdl_slots = 0;
 
     // ---- flush: ship the staged mutations to HBM on the side stream WITHOUT stopping the matches ------------------------
     // Phase A (no fence; only the host-mirror lock `mu` is held, matches keep running):
@@ -277,8 +281,8 @@ struct gm_engine {
             jobs_.clear(); swaps_.clear(); stage_used_ = 0;               // (fresh buffers not yet swapped in are freed here)
             up_ranges = up_values = up_pool = 0; up_edges_slots = up_dict_slots = 0;
             trie.full_edges = trie.full_dict = true; trie.cfilter_dirty = true; trie.trees_dirty = true; trie.root_dirty = true;
-            up_rkids = up_rvals = up_redges_slots = 0;
-            rtree.dirty = true; rtree.full = true;
+            up_rkids = up_rvals = up_redges_slots = up_rdl_slots = 0;
+            rtree.dirty = true; rtree.full = true; rtree.full_dl = true;
         }
         return st;
     }
@@ -314,6 +318,7 @@ struct gm_engine {
                 GM_TRY(upload_table(d_redges, rtree.redges, full_edges, rtree.dirty_edges, up_redges_slots));
                 GM_TRY(upload_appendable(d_rvals, rtree.rvals, up_rvals, &rtree.dirty_vals));
             }
+            if (!rtree.dl.empty()) GM_TRY(upload_table(d_rdl, rtree.dl, rtree.full_dl, rtree.dirty_dl, up_rdl_slots));   // whole when it grew
             r_shipped = true;
         }
         GM_TRY(upload_table(d_edges, trie.edges, trie.full_edges, trie.dirty_edges, up_edges_slots));
@@ -358,6 +363,7 @@ struct gm_engine {
             dev_view = trie_view(trie, d_edges.as<EdgeSlot>(), d_ranges.as<Range>(), d_values.as<u32>(), d_dict.as<DictSlot>(), d_pool.as<u8>(), d_cfilter.as<u32>(),
                                  d_tree_slots.as<u32>());
             dev_rview = retain_view(rtree, d_rkids.as<RKid>(), d_redges.as<REdge>(), d_rvals.as<u32>());
+            if (r_shipped) dev_rdl_n = rtree.dl_lookup_size();
             view_epoch++;
             CUDA_TRY(cudaEventRecord(ev_flush, side));
         }
@@ -436,8 +442,10 @@ struct gm_engine {
     }
     // `hdr` (small-graph form, small_graph_retain): n is the capacity and the caller holds mu_dev while it captures — no waits
     // on other streams' events, no completion or timing events (the caller orders the graph launch itself)
+    // With deadlines on the engine the lookup is evaluated at `now_ms`: a small graph reads it from hdr[2..3], the pipelined
+    // lookup from d_rnow (copied from pinned memory on `s`; mu_ret keeps it until the lookup is done).
     int enqueue_retain(const void* d_blob_, u64 blob_bytes, const u32* d_offs_, u64 n, gm_span* d_spans_, u32* d_ids_, u64 cap_ids, int32_t* d_status_, cudaStream_t s,
-                       const u32* hdr = nullptr) {
+                       u64 now_ms, const u32* hdr = nullptr) {
         std::unique_lock<std::mutex> gd(mu_dev, std::defer_lock);     // enqueue only; the caller (holding mu_ret) synchronises afterwards without it
         if (!hdr) gd.lock();
         MatchCtx& c = devctx;
@@ -450,16 +458,28 @@ struct gm_engine {
         }
         CUDA_TRY(cudaMemsetAsync(d_rctl.p, 0, p.ctl, s));
         CUDA_TRY(cudaMemsetAsync(d_rq.p, 0, p.rq, s));
+        RetainDeadlines x;
+        if (dev_rdl_n) {
+            x.dl = d_rdl.as<u64>(); x.n = dev_rdl_n;
+            if (hdr) x.now = reinterpret_cast<const u64*>(hdr + 2);
+            else {
+                CUDA_TRY(d_rnow.ensure(sizeof(u64)));
+                CUDA_TRY(h_rnow.ensure(sizeof(u64)));
+                *h_rnow.as<u64>() = now_ms;
+                CUDA_TRY(cudaMemcpyAsync(d_rnow.p, h_rnow.p, sizeof(u64), cudaMemcpyHostToDevice, s));
+                x.now = d_rnow.as<u64>();
+            }
+        }
         const bool timing = hdr == nullptr;
         const Event* ev_t = ev_ring[ring_n % RING];
         cudaError_t ev = cudaSuccess;
-        launch_retain(p, r, dev_view, dev_rview, d_blob_, blob_bytes, d_offs_, d_spans_, d_ids_, cap_ids, d_status_, knobs.retain_stats && !hdr, s, hdr,
+        launch_retain(p, r, dev_view, dev_rview, d_blob_, blob_bytes, d_offs_, d_spans_, d_ids_, cap_ids, d_status_, knobs.retain_stats && !hdr, s, hdr, x,
                       [&](int k) { if (timing && ev == cudaSuccess) ev = cudaEventRecord(ev_t[k], s); });
         CUDA_TRY(ev);
         CUDA_TRY(cudaGetLastError());
         if (!hdr) {
             ring_n++;
-            launches += 4 + p.depth + 1;
+            launches += 4 + p.depth + 1 + (x.n ? 1 : 0);
             CUDA_TRY(cudaEventRecord(c.ev_done, s));
             c.recorded = true;
         }
@@ -467,9 +487,10 @@ struct gm_engine {
     }
 
     // runs the pipeline, growing the frontier / descriptor scratch until nothing overflowed; leaves *total
-    int run_retain(const void* d_blob_, u64 blob_bytes, const u32* d_offs_, u64 n, gm_span* d_spans_, u32* d_ids_, u64 cap_ids, int32_t* d_status_, cudaStream_t s, u64* total) {
+    int run_retain(const void* d_blob_, u64 blob_bytes, const u32* d_offs_, u64 n, gm_span* d_spans_, u32* d_ids_, u64 cap_ids, int32_t* d_status_, cudaStream_t s, u64* total,
+                   u64 now_ms) {
         for (int attempt = 0; attempt < 12; ++attempt) {
-            GM_TRY(enqueue_retain(d_blob_, blob_bytes, d_offs_, n, d_spans_, d_ids_, cap_ids, d_status_, s));
+            GM_TRY(enqueue_retain(d_blob_, blob_bytes, d_offs_, n, d_spans_, d_ids_, cap_ids, d_status_, s, now_ms));
             RCtl h{};
             CUDA_TRY(cudaMemcpyAsync(&h, d_rctl.p, sizeof(RCtl), cudaMemcpyDeviceToHost, s));
             CUDA_TRY(cudaStreamSynchronize(s));
@@ -711,7 +732,7 @@ static int small_graph_tier(u64 n, u64 blob_bytes) {
     return -1;
 }
 
-// in-block:  {n, text bytes} (16 B) | offsets [cap_n + 1] | trees [cap_n] | text (256-aligned)
+// in-block:  {n, text bytes, u64 now: a retained lookup's clock with deadlines} (16 B) | offsets [cap_n + 1] | trees [cap_n] | text (256-aligned)
 // out-block: head (32 B: the match's cursor, or the retained lookup's RCtl head) | spans [cap_n] | status [cap_n] | output (256-aligned)
 static int small_graph_new(std::unique_ptr<SmallGraph>& slot, int tier) {
     auto g = std::make_unique<SmallGraph>();
@@ -822,7 +843,7 @@ static int small_graph_match(gm_engine* e, MatchCtx& c, std::unique_lock<std::mu
 // a tier, a frontier or descriptor overflow, or more ids than the tier holds — the caller runs the pipelined lookup, which
 // grows the scratch and returns the same results.
 static int small_graph_retain(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, gm_span* out_spans, uint32_t* out_ids, uint64_t cap_ids,
-                              uint64_t* needed, int32_t* status) {
+                              uint64_t* needed, int32_t* status, u64 now_ms) {
     const int tier = small_graph_tier(n, offsets[n] - offsets[0]);
     if (tier < 0) return GM_SMALL_NOT_APPLICABLE;
     std::unique_ptr<SmallGraph>& slot = e->rsmall[tier];
@@ -834,7 +855,7 @@ static int small_graph_retain(gm_engine* e, const char* blob, const uint32_t* of
         char* di = static_cast<char*>(g->d_in.p);
         char* dout = static_cast<char*>(g->d_out.p);
         int st = e->enqueue_retain(di + g->off_blob, g->cap_blob, reinterpret_cast<const u32*>(di + g->off_offs), g->cap_n, reinterpret_cast<gm_span*>(dout + g->off_spans),
-                                   reinterpret_cast<u32*>(dout + g->off_out), g->cap_out, reinterpret_cast<int32_t*>(dout + g->off_status), s, reinterpret_cast<const u32*>(di));
+                                   reinterpret_cast<u32*>(dout + g->off_out), g->cap_out, reinterpret_cast<int32_t*>(dout + g->off_status), s, 0, reinterpret_cast<const u32*>(di));
         if (st != GM_OK) return st;
         static_assert(offsetof(RCtl, err) + sizeof(u32) <= 32, "the out-block head holds RCtl up to err");
         CUDA_TRY(cudaMemcpyAsync(dout, e->d_rctl.p, 32, cudaMemcpyDeviceToDevice, s));
@@ -861,11 +882,12 @@ static int small_graph_retain(gm_engine* e, const char* blob, const uint32_t* of
     }
     GM_TRY(small_graph_refresh(g, c.sc, e->view_epoch, e->retain_sig(), sizeof(u32), enqueue));
     small_graph_fill(g, blob, offsets, n);
+    std::memcpy(g->h_in.p + 8, &now_ms, sizeof(u64));             // the in-block header's {now} (read only with deadlines)
     GM_TRY(order());
     CUDA_TRY(cudaGraphLaunch(g->exec, c.sc));
     CUDA_TRY(cudaEventRecord(c.ev_done, c.sc));
     c.recorded = true;
-    e->launches += 4 + e->dev_rview.max_depth + 1;
+    e->launches += 4 + e->dev_rview.max_depth + 1 + (e->dev_rdl_n ? 1 : 0);
     gd.unlock();
     CUDA_TRY(cudaStreamSynchronize(c.sc));
     RCtl head;
@@ -1019,14 +1041,39 @@ int32_t gm_desc_expand(gm_engine* e, const gm_desc* descs, uint64_t n, uint32_t*
 }
 
 // ---- retained-message tree ----------------------------------------------------------------------------
-int32_t gm_retain_set(gm_engine* e, const char* topic, uint32_t len, uint32_t value, int32_t* had_old, uint32_t* old_value) {
+static int32_t map_retain(int st, const char* what) {
+    if (st == RetainTreeHost::SET_CONFLICT) { g_err = std::string(what) + ": the handle carries a deadline under another topic"; return GM_ERR_INVALID_ARG; }
+    if (st == RetainTreeHost::SET_HANDLE_RANGE) { g_err = std::string(what) + ": handles with a deadline must be below GM_RETAIN_TTL_MAX_HANDLE"; return GM_ERR_INVALID_ARG; }
+    return map_parse(st, what);
+}
+
+// the wall clock in the unit of deadlines: ms since the Unix epoch (rmqtt's timestamp_millis)
+static u64 wall_ms() { return static_cast<u64>(std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::system_clock::now().time_since_epoch()).count()); }
+
+static int32_t retain_set_impl(gm_engine* e, const char* topic, uint32_t len, uint32_t value, uint64_t deadline_ms, int32_t* had_old, uint32_t* old_value, const char* what) {
     if (!e || (!topic && len)) return GM_ERR_INVALID_ARG;
     std::lock_guard<std::mutex> g(e->mu);
     bool had = false; u32 old = 0;
-    int st = e->rtree.set(topic, len, value, &had, &old);
+    int st = e->rtree.set_ttl(topic, len, value, deadline_ms, &had, &old);
     if (had_old) *had_old = had ? 1 : 0;
     if (old_value && had) *old_value = old;
-    return map_parse(st, "gm_retain_set");
+    return map_retain(st, what);
+}
+
+int32_t gm_retain_set(gm_engine* e, const char* topic, uint32_t len, uint32_t value, int32_t* had_old, uint32_t* old_value) {
+    return retain_set_impl(e, topic, len, value, 0, had_old, old_value, "gm_retain_set");
+}
+
+int32_t gm_retain_set_ttl(gm_engine* e, const char* topic, uint32_t len, uint32_t value, uint64_t deadline_ms, int32_t* had_old, uint32_t* old_value) {
+    return retain_set_impl(e, topic, len, value, deadline_ms, had_old, old_value, "gm_retain_set_ttl");
+}
+
+int32_t gm_retain_remove_expired(gm_engine* e, uint64_t now_ms, uint32_t* out_values, uint64_t cap, uint64_t* n_removed) {
+    if (!e || (cap && !out_values)) return GM_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> g(e->mu);
+    const u64 n = e->rtree.remove_expired(now_ms, out_values, cap);
+    if (n_removed) *n_removed = n;
+    return GM_OK;
 }
 
 int32_t gm_retain_remove(gm_engine* e, const char* topic, uint32_t len, int32_t* had_old, uint32_t* old_value) {
@@ -1036,7 +1083,7 @@ int32_t gm_retain_remove(gm_engine* e, const char* topic, uint32_t len, int32_t*
     int st = e->rtree.remove(topic, len, &had, &old);
     if (had_old) *had_old = had ? 1 : 0;
     if (old_value && had) *old_value = old;
-    return map_parse(st, "gm_retain_remove");
+    return map_retain(st, "gm_retain_remove");
 }
 
 int32_t gm_retain_remove_batch(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, uint32_t* old_values, uint64_t* n_removed) {
@@ -1053,16 +1100,29 @@ int32_t gm_retain_remove_batch(gm_engine* e, const char* blob, const uint32_t* o
     return GM_OK;
 }
 
-int32_t gm_retain_bulk_load(gm_engine* e, const char* blob, const uint32_t* offsets, const uint32_t* values, uint64_t n, uint64_t* n_set) {
+static int32_t retain_bulk_impl(gm_engine* e, const char* blob, const uint32_t* offsets, const uint32_t* values, const uint64_t* deadlines, uint64_t n, uint64_t* n_set,
+                                const char* what) {
     if (!e || (n && (!blob || !offsets || !values))) return GM_ERR_INVALID_ARG;
     std::lock_guard<std::mutex> g(e->mu);
-    const uint64_t ok = e->rtree.set_batch(blob, offsets, values, n);
+    GM_TRY(map_retain(e->rtree.check_batch(blob, offsets, values, deadlines, n), what));
+    const uint64_t ok = deadlines ? e->rtree.set_batch_ttl(blob, offsets, values, deadlines, n) : e->rtree.set_batch(blob, offsets, values, n);
     if (n_set) *n_set = ok;
     return GM_OK;
 }
 
+int32_t gm_retain_bulk_load(gm_engine* e, const char* blob, const uint32_t* offsets, const uint32_t* values, uint64_t n, uint64_t* n_set) {
+    return retain_bulk_impl(e, blob, offsets, values, nullptr, n, n_set, "gm_retain_bulk_load");
+}
+
+int32_t gm_retain_bulk_load_ttl(gm_engine* e, const char* blob, const uint32_t* offsets, const uint32_t* values, const uint64_t* deadlines_ms, uint64_t n,
+                                uint64_t* n_set) {
+    if (n && !deadlines_ms) return GM_ERR_INVALID_ARG;
+    return retain_bulk_impl(e, blob, offsets, values, deadlines_ms, n, n_set, "gm_retain_bulk_load_ttl");
+}
+
 int32_t gm_retain_match_batch_device(gm_engine* e, const void* d_blob, uint64_t blob_bytes, const uint32_t* d_offs, uint64_t n,
                                      gm_span* d_spans, uint32_t* d_ids, uint64_t cap_ids, uint64_t* needed, int32_t* d_status, void* stream) {
+    const u64 now_ms = wall_ms();
     if (!e || (n && (!d_offs || !d_spans || !d_status))) return GM_ERR_INVALID_ARG;
     if (needed) *needed = 0;
     if (n == 0) return GM_OK;
@@ -1072,7 +1132,7 @@ int32_t gm_retain_match_batch_device(gm_engine* e, const void* d_blob, uint64_t 
     std::lock_guard<std::mutex> gr(e->mu_ret);      // the retained lookup's scratch is engine-wide: one lookup at a time
     GM_TRY(auto_flush(e, true));
     u64 total = 0;
-    GM_TRY(e->run_retain(d_blob, blob_bytes, d_offs, n, d_spans, d_ids, std::min<u64>(cap_ids, 0xFFFFFFFFull), d_status, static_cast<cudaStream_t>(stream), &total));
+    GM_TRY(e->run_retain(d_blob, blob_bytes, d_offs, n, d_spans, d_ids, std::min<u64>(cap_ids, 0xFFFFFFFFull), d_status, static_cast<cudaStream_t>(stream), &total, now_ms));
     if (needed) *needed = total;
     if (total > 0xFFFFFFFFull) { g_err = "batch produces >= 2^32 ids: split it"; return GM_ERR_TOO_LARGE; }
     if (total > cap_ids) { g_err = "out_ids too small"; return GM_ERR_CAPACITY; }
@@ -1081,6 +1141,11 @@ int32_t gm_retain_match_batch_device(gm_engine* e, const void* d_blob, uint64_t 
 
 int32_t gm_retain_match_batch(gm_engine* e, const char* blob, const uint32_t* offsets, uint64_t n, gm_span* out_spans, uint32_t* out_ids,
                               uint64_t cap_ids, uint64_t* needed, int32_t* status) {
+    return gm_retain_match_batch_at(e, wall_ms(), blob, offsets, n, out_spans, out_ids, cap_ids, needed, status);
+}
+
+int32_t gm_retain_match_batch_at(gm_engine* e, uint64_t now_ms, const char* blob, const uint32_t* offsets, uint64_t n, gm_span* out_spans, uint32_t* out_ids,
+                                 uint64_t cap_ids, uint64_t* needed, int32_t* status) {
     if (!e || (n && (!offsets || !out_spans || !status)) || (cap_ids && !out_ids)) return GM_ERR_INVALID_ARG;
     if (needed) *needed = 0;
     if (n == 0) return GM_OK;
@@ -1090,7 +1155,7 @@ int32_t gm_retain_match_batch(gm_engine* e, const char* blob, const uint32_t* of
     std::lock_guard<std::mutex> gr(e->mu_ret);
     GM_TRY(auto_flush(e, true));
     if (e->knobs.small_graphs && !e->knobs.retain_stats) {      // (the per-round diagnostics come from the pipelined path)
-        int st = small_graph_retain(e, blob, offsets, n, out_spans, out_ids, cap_ids, needed, status);
+        int st = small_graph_retain(e, blob, offsets, n, out_spans, out_ids, cap_ids, needed, status, now_ms);
         if (st != GM_SMALL_NOT_APPLICABLE) return st;
     }
     const u64 blob_bytes = offsets[n];
@@ -1106,7 +1171,7 @@ int32_t gm_retain_match_batch(gm_engine* e, const char* blob, const uint32_t* of
     CUDA_TRY(cudaMemcpyAsync(ro.p, offsets, (n + 1) * sizeof(u32), cudaMemcpyHostToDevice, s));
     u64 total = 0;
     int st = e->run_retain(rb.p, blob_bytes, ro.as<u32>(), n, rs.as<gm_span>(), ri.as<u32>(), std::min<u64>(cap_ids, 0xFFFFFFFFull),
-                           rt.as<int32_t>(), s, &total);
+                           rt.as<int32_t>(), s, &total, now_ms);
     if (st != GM_OK) return st;
     CUDA_TRY(cudaMemcpyAsync(status, rt.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(out_spans, rs.p, n * sizeof(gm_span), cudaMemcpyDeviceToHost, s));

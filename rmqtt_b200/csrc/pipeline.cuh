@@ -212,12 +212,18 @@ inline void launch_match(const MatchPlan& p, const MatchScratch& m, const MatchI
 
 struct RetainScratch { u32 *tok, *tok8, *meta, *rq; RCtl* ctl; RTask* front[2]; RDesc* descs; };
 
+// The deadlines a retained lookup honours: the shipped handle-indexed table (~0 = none) and the lookup's `now` (ms since the
+// Unix epoch) in device memory.  n == 0: the engine holds no deadline, and the lookup runs the plain kernels.
+struct RetainDeadlines { const u64* dl = nullptr; u32 n = 0; const u64* now = nullptr; };
+
 // k_tokenize -> k_retain_init -> k_retain_round x (depth + 1) -> k_retain_scan -> k_retain_expand.  `at(k)` runs before the
 // tokeniser (0), after it (1), after the last round (2) and after the expansion (3).  `hdr` (small-graph form, as MatchIO::hdr):
 // {n, blob_bytes} in memory, read at run time; p.nq is then the capacity.  Without it the launch is the pipelined lookup of nq filters.
+// With deadlines (x.n > 0) the walk and the expansion are the TTL instantiations and k_retain_live runs before the scan.
 template <class Hook = NoHook>
 inline void launch_retain(const RetainPlan& p, const RetainScratch& r, const TrieView& tv, const RetainView& rv, const void* blob, u64 blob_bytes, const u32* offs,
-                          gm_span* spans, u32* ids, u64 cap_ids, int32_t* status, bool stats, cudaStream_t s, const u32* hdr = nullptr, Hook at = {}) {
+                          gm_span* spans, u32* ids, u64 cap_ids, int32_t* status, bool stats, cudaStream_t s, const u32* hdr = nullptr,
+                          const RetainDeadlines& x = {}, Hook at = {}) {
     const u32 nq = p.nq, depth = p.depth;
     u32* qtotal = r.rq;
     u32* qbase = qtotal + nq;
@@ -231,17 +237,21 @@ inline void launch_retain(const RetainPlan& p, const RetainScratch& r, const Tri
     rp.descs = r.descs; rp.n_desc = r.ctl->n_desc; rp.cap_items = p.slice_items; rp.cap_desc = p.slice_desc;
     rp.qtotal = qtotal; rp.err = &r.ctl->err;
     rp.stats = r.ctl->stats;
+    rp.dl = x.dl; rp.n_dl = x.n; rp.now = x.now;
+    const bool ttl = x.n > 0;
     // round 0 follows every filter's literal prefix; every later round expands the wildcard tasks the round before
     // queued.  A task descends at least one tree level, so depth + 1 rounds drain every queue (late rounds find
     // theirs empty and return at once).
-    auto kri = stats ? k_retain_init<true> : k_retain_init<false>;
-    auto krr = stats ? k_retain_round<true> : k_retain_round<false>;
+    auto kri = ttl ? (stats ? k_retain_init<true, true> : k_retain_init<false, true>) : (stats ? k_retain_init<true, false> : k_retain_init<false, false>);
+    auto krr = ttl ? (stats ? k_retain_round<true, true> : k_retain_round<false, true>) : (stats ? k_retain_round<true, false> : k_retain_round<false, false>);
     GM_LAUNCH(kri, p.init_grid, 256, 0, s, rp, r.front[0], r.ctl->round_counts(0));
     for (u32 lvl = 0; lvl <= depth; ++lvl)
         GM_LAUNCH(krr, p.round_grid, 256, 0, s, rp, r.front[lvl & 1], r.ctl->round_counts(lvl), r.front[(lvl + 1) & 1], r.ctl->round_counts(lvl + 1), r.ctl->claim(depth, lvl));
     at(2);
+    if (ttl) GM_LAUNCH(k_retain_live, p.expand_grid, 256, 0, s, r.descs, r.ctl->n_desc, p.slice_desc, rv.vals, qtotal, x.dl, x.n, x.now);
     GM_LAUNCH(k_retain_scan, 1, 1024, 0, s, qtotal, nq, hdr, qbase, reinterpret_cast<uint2*>(spans), &r.ctl->grand);
-    GM_LAUNCH(k_retain_expand, p.expand_grid, 256, 0, s, r.descs, r.ctl->n_desc, p.slice_desc, rv.vals, qbase, qcur, ids, cap_ids);
+    auto kre = ttl ? k_retain_expand<true> : k_retain_expand<false>;
+    GM_LAUNCH(kre, p.expand_grid, 256, 0, s, r.descs, r.ctl->n_desc, p.slice_desc, rv.vals, qbase, qcur, ids, cap_ids, x.dl, x.n, x.now);
     at(3);
 }
 

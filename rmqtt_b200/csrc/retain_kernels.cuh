@@ -45,7 +45,16 @@ struct RetainParams {
     u32* qtotal;         // [nq] matched values per query
     u32* err;            // bit 0: task-queue overflow, bit 1: descriptor overflow
     unsigned long long* stats;   // optional [2]: nodes visited, hash probes issued (diagnostics)
+    // Deadlines (read by the TTL instantiations only; kept last so that the other instantiations see an unchanged layout):
+    // dl[handle] in ms since the Unix epoch, ~0 = none; handles at or past n_dl never expire.  `now` lives in device memory,
+    // so a captured graph reads the current one at every launch.
+    const u64* dl;
+    u32 n_dl;
+    const u64* now;
 };
+
+// a handle is live at `now` unless its deadline has come (TimedValue::is_expired: now >= deadline)
+__device__ __forceinline__ bool retain_live(const u64* dl, u32 n_dl, u64 now, u32 v) { return v >= n_dl || now < dl[v]; }
 
 __device__ __forceinline__ u32 retain_tok(const RetainParams& p, u32 q, u32 pos) {
     return pos < TOK8 ? p.qtok8[static_cast<size_t>(q) * TOK8 + pos] : p.qtok[static_cast<size_t>(pos) * p.nq + q];
@@ -86,6 +95,11 @@ __device__ __forceinline__ void emit_desc(const RetainParams& p, u32 sq, u32 q, 
     const u32 at = atomicAdd(p.n_desc + sq, 1u);
     if (at < p.cap_desc) p.descs[static_cast<size_t>(sq) * p.cap_desc + at] = RDesc{q, ref, cnt, kind}; else atomicOr(p.err, 2u);
 }
+// one matched value: with deadlines, an expired one is neither counted nor recorded
+template <bool TTL>
+__device__ __forceinline__ void emit_value(const RetainParams& p, u64 now, u32 sq, u32 q, u32 v) {
+    if (!TTL || retain_live(p.dl, p.n_dl, now, v)) emit_desc(p, sq, q, v, 1u, 0u);
+}
 // LOCALITY: a task goes into the queue slice of its child block's POSITION IN THE TREE (child blocks are laid out in tree
 // pre-order), not of the warp that produced it.  The next round consumes the slices one after another, so all the tasks
 // that expand the same part of the tree — dozens of filters such as `+/+/+/…` and `reg/+/+/…` cover every site block — run
@@ -116,8 +130,8 @@ struct RRec { u32 node, first_kid, nk_flags, val, val_lo, val_hi, mask; };
 // 838 K of the 1.02 M tasks of a batch had 1..5 children (a device's sensors, a sensor's metrics), and a task costs a
 // queue record, a warp and ~500 warp-instructions of bookkeeping whatever its size.
 constexpr u32 RINLINE_KIDS = 8, RINLINE_DEPTH = 4;
-template <bool STATS>
-__device__ __forceinline__ void retain_chain(const RetainParams& p, RTask* out, u32* n_out, u32 sq, u32 q, u32 L, u32 pos, RRec r,
+template <bool STATS, bool TTL>
+__device__ __forceinline__ void retain_chain(const RetainParams& p, u64 now, RTask* out, u32* n_out, u32 sq, u32 q, u32 L, u32 pos, RRec r,
                                              unsigned long long& visited, unsigned long long& probes) {
     const RetainView& v = p.v;
     u32 st_kb[RINLINE_DEPTH], st_ke[RINLINE_DEPTH], st_pm[RINLINE_DEPTH];     // child range still to visit, pos | mode << 30
@@ -129,7 +143,7 @@ __device__ __forceinline__ void retain_chain(const RetainParams& p, RTask* out, 
             if (STATS) ++visited;
             const u32 nkids = r.nk_flags & RNK_MASK, flags = r.nk_flags >> 28;
             if (nkids == 0 || pos == L) {                                        // retain.rs:305-311
-                if (pos == L && (flags & 8u)) emit_desc(p, sq, q, r.val, 1u, 0u);
+                if (pos == L && (flags & 8u)) emit_value<TTL>(p, now, sq, q, r.val);
                 break;
             }
             const u32 tok = retain_tok(p, q, pos);
@@ -141,7 +155,7 @@ __device__ __forceinline__ void retain_chain(const RetainParams& p, RTask* out, 
             bool found = false;
             if (exact_try && (r.mask & retain_mask_bit(tok))) { if (STATS) ++probes; found = retain_child(v, r.node, tok, c); }
             if (found) {
-                if (next_hash && ((c[4] >> 28) & 8u)) emit_desc(p, sq, q, c[5], 1u, 0u);   // '#' matches the parent, retain.rs:317-322
+                if (next_hash && ((c[4] >> 28) & 8u)) emit_value<TTL>(p, now, sq, q, c[5]);   // '#' matches the parent, retain.rs:317-322
                 r = RRec{c[2], c[3], c[4], c[5], c[6], c[7], 0xFFFFFFFFu};
                 ++pos;
                 descend = true;
@@ -174,12 +188,12 @@ __device__ __forceinline__ void retain_chain(const RetainParams& p, RTask* out, 
             const u32 kkids = kd[3] & RNK_MASK;
             if (STATS) ++visited;
             if (fmode == 1u) {
-                if (fpos + 1 == L) { if (has_val) emit_desc(p, sq, q, kd[4], 1u, 0u); continue; }
-                if (has_val && (fpos + 1 < L) && retain_tok(p, q, fpos + 1) == TOK_HASH) emit_desc(p, sq, q, kd[4], 1u, 0u);   // `.../+/#` parent match
+                if (fpos + 1 == L) { if (has_val) emit_value<TTL>(p, now, sq, q, kd[4]); continue; }
+                if (has_val && (fpos + 1 < L) && retain_tok(p, q, fpos + 1) == TOK_HASH) emit_value<TTL>(p, now, sq, q, kd[4]);   // `.../+/#` parent match
                 if (!kkids) continue;
                 pos = fpos + 1;
             } else {
-                if (has_val) emit_desc(p, sq, q, kd[4], 1u, 0u);
+                if (has_val) emit_value<TTL>(p, now, sq, q, kd[4]);
                 if (!kkids) continue;
                 pos = fpos;
             }
@@ -191,16 +205,17 @@ __device__ __forceinline__ void retain_chain(const RetainParams& p, RTask* out, 
 }
 
 // round 0: one thread per query walks the literal prefix of its filter from the root
-template <bool STATS>
+template <bool STATS, bool TTL>
 __global__ void __launch_bounds__(256)
 k_retain_init(RetainParams p, RTask* out, u32* n_out) {
     const u32 q = blockIdx.x * blockDim.x + threadIdx.x;
     const u32 n_act = p.n_ptr ? min(p.nq, *p.n_ptr) : p.nq;
+    const u64 now = TTL ? *p.now : 0ull;
     unsigned long long visited = 0, probes = 0;
     if (q < n_act) {
         const u32 m = p.qmeta[q];
         if (!(m & META_INVALID))
-            retain_chain<STATS>(p, out, n_out, (q >> 5) % RQ, q, m & META_NLEV_MASK, 0u,
+            retain_chain<STATS, TTL>(p, now, out, n_out, (q >> 5) % RQ, q, m & META_NLEV_MASK, 0u,
                                 RRec{0u, p.v.root_first_kid, p.v.root_nk_flags, 0u, 0u, p.v.root_plain_val_hi, 0xFFFFFFFFu}, visited, probes);
     }
     if (STATS && (visited | probes)) { atomicAdd(p.stats, visited); atomicAdd(p.stats + 1, probes); }
@@ -217,7 +232,7 @@ constexpr u32 RLIST = 256;    // = RTASK_CHUNK: at most one survivor per child o
 #ifndef GM_RETAIN_CTAS
 #define GM_RETAIN_CTAS 6
 #endif
-template <bool STATS>
+template <bool STATS, bool TTL>
 __global__ void __launch_bounds__(256, GM_RETAIN_CTAS)
 k_retain_round(RetainParams p, const RTask* __restrict__ in, const u32* __restrict__ n_in_p, RTask* __restrict__ out, u32* n_out, u32* __restrict__ claim) {
     static_assert(RLIST >= RTASK_CHUNK, "the survivor list holds one entry per child of a task");
@@ -227,6 +242,7 @@ k_retain_round(RetainParams p, const RTask* __restrict__ in, const u32* __restri
     __shared__ u32 s_pre[RQ + 1];
     __shared__ u32 s_list[8][2][RLIST];
     const u32 n_in = queue_prefix(n_in_p, p.cap_items, s_pre);
+    const u64 now = TTL ? *p.now : 0ull;
     const u32 sq = gwarp % RQ;                        // this warp appends to its own slice
     unsigned long long visited = 0, probes = 0;
     // tasks differ in size by two orders of magnitude (1 .. 256 children, 0 .. 3 probe levels below): warps CLAIM them one
@@ -258,18 +274,18 @@ k_retain_round(RetainParams p, const RTask* __restrict__ in, const u32* __restri
                 const u32 kkids = kd[3] & RNK_MASK;
                 bool go = false;
                 if (mode == 1u) {
-                    if (pos + 1 == L) { if (has_val) emit_desc(p, sq, q, kd[4], 1u, 0u); }   // filter ends here: the child's own value
+                    if (pos + 1 == L) { if (has_val) emit_value<TTL>(p, now, sq, q, kd[4]); }   // filter ends here: the child's own value
                     else {
-                        if (next_hash && has_val) emit_desc(p, sq, q, kd[4], 1u, 0u);        // `.../+/#` parent match
+                        if (next_hash && has_val) emit_value<TTL>(p, now, sq, q, kd[4]);        // `.../+/#` parent match
                         go = kkids != 0;
                     }
                 } else {                                            // '#' one level at a time (a literal "#" child hides below)
-                    if (has_val) emit_desc(p, sq, q, kd[4], 1u, 0u);
+                    if (has_val) emit_value<TTL>(p, now, sq, q, kd[4]);
                     go = kkids != 0;
                 }
                 if (go) {
                     if (tokP >= TOK_BLANK) { want = (kd[7] & retain_mask_bit(tokP)) != 0; wnode = kd[1]; }   // exact level: lock-step list
-                    else retain_chain<STATS>(p, out, n_out, sq, q, L, P, RRec{kd[1], kd[2], kd[3], kd[4], kd[5], kd[6], kd[7]}, visited, probes);
+                    else retain_chain<STATS, TTL>(p, now, out, n_out, sq, q, L, P, RRec{kd[1], kd[2], kd[3], kd[4], kd[5], kd[6], kd[7]}, visited, probes);
                 }
             }
             const u32 bal = __ballot_sync(0xFFFFFFFFu, want);
@@ -292,10 +308,10 @@ k_retain_round(RetainParams p, const RTask* __restrict__ in, const u32* __restri
                     if (STATS) { ++probes; ++visited; }
                     if (retain_child(v, node, tokP, c)) {
                         const u32 fl = c[4] >> 28, nk = c[4] & RNK_MASK;
-                        if (nh && (fl & 8u)) emit_desc(p, sq, q, c[5], 1u, 0u);              // '#' matches the parent, retain.rs:317-322
-                        if (nk == 0 || P1 == L) { if (P1 == L && (fl & 8u)) emit_desc(p, sq, q, c[5], 1u, 0u); }   // retain.rs:305-311
+                        if (nh && (fl & 8u)) emit_value<TTL>(p, now, sq, q, c[5]);              // '#' matches the parent, retain.rs:317-322
+                        if (nk == 0 || P1 == L) { if (P1 == L && (fl & 8u)) emit_value<TTL>(p, now, sq, q, c[5]); }   // retain.rs:305-311
                         else if (tok1 >= TOK_BLANK) { want = true; wnode = c[2]; }             // another exact level (a hash slot has no mask)
-                        else retain_chain<STATS>(p, out, n_out, sq, q, L, P1, RRec{c[2], c[3], c[4], c[5], c[6], c[7], 0xFFFFFFFFu}, visited, probes);
+                        else retain_chain<STATS, TTL>(p, now, out, n_out, sq, q, L, P1, RRec{c[2], c[3], c[4], c[5], c[6], c[7], 0xFFFFFFFFu}, visited, probes);
                     }
                 }
                 const u32 bal = __ballot_sync(0xFFFFFFFFu, want);
@@ -342,24 +358,76 @@ k_retain_scan(const u32* __restrict__ qtotal, u32 nq, const u32* __restrict__ n_
     }
 }
 
-// Expands the descriptors into per-query contiguous lists (load-balanced like the publish step of k_match_fast).
+// lanes [a, b) of a warp (0 <= a <= b <= 32, a < 32)
+__device__ __forceinline__ u32 lane_range(u32 a, u32 b) { return (b >= 32 ? 0xFFFFFFFFu : (1u << b) - 1u) & ~((1u << a) - 1u); }
+
+// With deadlines only, between the last round and k_retain_scan: a '#' range descriptor (kind 1) counted every value of its
+// range in qtotal.  This pass subtracts the expired ones and keeps the range's live count in the descriptor
+// (kind = 1 | live << 1) for k_retain_expand.  Load-balanced like the expansion: a warp takes 32 descriptors and reads their
+// ranges 32 values per step; every descriptor's lane counts the expired values of its own run in the step's ballot.
 __global__ void __launch_bounds__(256)
-k_retain_expand(const RDesc* __restrict__ descs, const u32* __restrict__ n_desc_p, u32 cap_desc, const u32* __restrict__ rvals,
-                const u32* __restrict__ qbase, u32* __restrict__ qcur, u32* __restrict__ out, unsigned long long cap_ids) {
+k_retain_live(RDesc* __restrict__ descs, const u32* __restrict__ n_desc_p, u32 cap_desc, const u32* __restrict__ rvals, u32* __restrict__ qtotal,
+              const u64* __restrict__ dl, u32 n_dl, const u64* __restrict__ now_p) {
     const u32 lane = threadIdx.x & 31;
     const u32 gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
     __shared__ u32 s_pre[RQ + 1];
     const u32 nd = queue_prefix(n_desc_p, cap_desc, s_pre);
+    const u64 now = *now_p;
     for (u32 base = gwarp * 32; base < nd; base += nwarps * 32) {
         const u32 i = base + lane;
-        RDesc d = i < nd ? descs[queue_locate(s_pre, i, cap_desc)] : RDesc{0, 0, 0, 0};
-        const u32 ni = d.cnt;
-        const u32 dst = ni ? qbase[d.q] + atomicAdd(qcur + d.q, ni) : 0u;
+        const size_t at = i < nd ? queue_locate(s_pre, i, cap_desc) : 0;
+        const RDesc d = i < nd ? descs[at] : RDesc{0, 0, 0, 0};
+        const u32 ni = d.kind == 1u ? d.cnt : 0u;                // single values were checked where they were emitted
         u32 sc = ni;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { u32 x = __shfl_up_sync(0xFFFFFFFFu, sc, o); if (lane >= o) sc += x; }
         const u32 tot = __shfl_sync(0xFFFFFFFFu, sc, 31);
         const u32 exc = sc - ni;
+        u32 dead = 0;
+        for (u32 e0 = 0; e0 < tot; e0 += 32) {
+            const u32 e = e0 + lane;
+            const u32 lo = warp_run_owner(exc, e);
+            const u32 o_exc = __shfl_sync(0xFFFFFFFFu, exc, lo);
+            const u32 o_ref = __shfl_sync(0xFFFFFFFFu, d.ref, lo);
+            const bool x = e < tot && !retain_live(dl, n_dl, now, rvals[o_ref + (e - o_exc)]);
+            const u32 bal = __ballot_sync(0xFFFFFFFFu, x);
+            const u32 a = max(exc, e0), b = min(exc + ni, e0 + 32u);
+            if (b > a) dead += __popc(bal & lane_range(a - e0, b - e0));
+        }
+        __syncwarp();      // no lane leaves before every lane took the last ballot (the CPU emulation drops exited lanes from it)
+        if (ni) {
+            if (dead) atomicAdd(qtotal + d.q, 0u - dead);       // (modular: subtracts)
+            descs[at].kind = 1u | ((ni - dead) << 1);
+        }
+    }
+}
+
+// Expands the descriptors into per-query contiguous lists (load-balanced like the publish step of k_match_fast).  TTL: the
+// ranges carry their live count (k_retain_live); expired values are compacted out with a warp ballot, so that every filter's
+// handles stay contiguous: a value goes to its descriptor's slot + the live values of its run in earlier steps + the live
+// lanes of its run before it in this step.
+template <bool TTL>
+__global__ void __launch_bounds__(256)
+k_retain_expand(const RDesc* __restrict__ descs, const u32* __restrict__ n_desc_p, u32 cap_desc, const u32* __restrict__ rvals,
+                const u32* __restrict__ qbase, u32* __restrict__ qcur, u32* __restrict__ out, unsigned long long cap_ids,
+                const u64* __restrict__ dl, u32 n_dl, const u64* __restrict__ now_p) {
+    const u32 lane = threadIdx.x & 31;
+    const u32 gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+    __shared__ u32 s_pre[RQ + 1];
+    const u32 nd = queue_prefix(n_desc_p, cap_desc, s_pre);
+    const u64 now = TTL ? *now_p : 0ull;
+    for (u32 base = gwarp * 32; base < nd; base += nwarps * 32) {
+        const u32 i = base + lane;
+        RDesc d = i < nd ? descs[queue_locate(s_pre, i, cap_desc)] : RDesc{0, 0, 0, 0};
+        const u32 ni = d.cnt;
+        const u32 nl = TTL && d.kind ? d.kind >> 1 : ni;        // slots to reserve: the live values
+        const u32 dst = nl ? qbase[d.q] + atomicAdd(qcur + d.q, nl) : 0u;
+        u32 sc = ni;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { u32 x = __shfl_up_sync(0xFFFFFFFFu, sc, o); if (lane >= o) sc += x; }
+        const u32 tot = __shfl_sync(0xFFFFFFFFu, sc, 31);
+        const u32 exc = sc - ni;
+        u32 run = 0;                                             // TTL: live values of this lane's descriptor written so far
         for (u32 e0 = 0; e0 < tot; e0 += 32) {
             const u32 e = e0 + lane;
             const u32 lo = warp_run_owner(exc, e);
@@ -367,12 +435,24 @@ k_retain_expand(const RDesc* __restrict__ descs, const u32* __restrict__ n_desc_
             const u32 o_ref = __shfl_sync(0xFFFFFFFFu, d.ref, lo);
             const u32 o_kind = __shfl_sync(0xFFFFFFFFu, d.kind, lo);
             const u32 o_dst = __shfl_sync(0xFFFFFFFFu, dst, lo);
-            if (e < tot) {
+            if (TTL) {
+                const u32 o_run = __shfl_sync(0xFFFFFFFFu, run, lo);
+                const u32 k = e - o_exc;
+                const u32 v = e < tot ? (o_kind ? rvals[o_ref + k] : o_ref) : 0u;
+                const bool live = e < tot && (!o_kind || retain_live(dl, n_dl, now, v));
+                const u32 bal = __ballot_sync(0xFFFFFFFFu, live);
+                const u32 first = o_exc > e0 ? o_exc - e0 : 0u;    // this run's first lane in the step
+                const unsigned long long at = static_cast<unsigned long long>(o_dst) + o_run + __popc(bal & lane_range(first, lane));
+                if (live && at < cap_ids) __stcs(out + at, v);
+                const u32 a = max(exc, e0), b = min(exc + ni, e0 + 32u);
+                if (b > a) run += __popc(bal & lane_range(a - e0, b - e0));
+            } else if (e < tot) {
                 const u32 k = e - o_exc;
                 const unsigned long long at = static_cast<unsigned long long>(o_dst) + k;
                 if (at < cap_ids) __stcs(out + at, o_kind ? rvals[o_ref + k] : o_ref);
             }
         }
+        if (TTL) __syncwarp();   // as in k_retain_live
     }
 }
 

@@ -5,6 +5,8 @@
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
+#include <functional>
+#include <string_view>
 
 #include "host_par.h"
 
@@ -20,7 +22,7 @@ u32 RetainTreeHost::child_of(u32 node, u32 token) const {
     return (it != k.end() && it->first == token) ? it->second : 0u;
 }
 
-int RetainTreeHost::set(const char* topic, u32 len, u32 value, bool* had_old, u32* old) {
+int RetainTreeHost::put(const char* topic, u32 len, u32 value, bool* had_old, u32* old) {
     if (had_old) *had_old = false;
     int st = parse(topic, len, true, toks_);
     if (st != PARSE_OK) return st;
@@ -67,6 +69,7 @@ int RetainTreeHost::remove(const char* topic, u32 len, bool* had_old, u32* old) 
     if (n.has_val) {
         if (had_old) *had_old = true;
         if (old) *old = n.val;
+        drop_deadline(n.val);
         n.has_val = false; n.val = RVAL_NONE;
         n_values_--;
         dirty = true;
@@ -90,6 +93,110 @@ int RetainTreeHost::remove(const char* topic, u32 len, bool* had_old, u32* old) 
         x = p;
     }
     return PARSE_OK;
+}
+
+int RetainTreeHost::set_ttl(const char* topic, u32 len, u32 value, u64 deadline, bool* had_old, u32* old) {
+    if (had_old) *had_old = false;
+    if (deadline && value >= DL_MAX_HANDLE) return SET_HANDLE_RANGE;
+    if (!dl_topic_.empty()) {
+        auto it = dl_topic_.find(value);
+        if (it != dl_topic_.end() && std::string_view(it->second) != std::string_view(topic, len)) return SET_CONFLICT;
+    }
+    bool had = false; u32 o = 0;
+    const int st = put(topic, len, value, &had, &o);
+    if (st != PARSE_OK) return st;
+    if (had_old) *had_old = had;
+    if (old && had) *old = o;
+    if (had && o != value) drop_deadline(o);
+    if (deadline) give_deadline(value, topic, len, deadline); else drop_deadline(value);
+    return PARSE_OK;
+}
+
+bool RetainTreeHost::holds(const char* topic, u32 len, u32 value) {
+    if (parse(topic, len, false, toks_) != PARSE_OK) return false;
+    u32 node = 0;
+    for (u32 tok : toks_) {
+        if (tok == TOK_UNKNOWN) return false;
+        if (!(node = child_of(node, tok))) return false;
+    }
+    return nodes_[node].has_val && nodes_[node].val == value;
+}
+
+void RetainTreeHost::give_deadline(u32 h, const char* topic, u32 len, u64 deadline) {
+    if (h >= dl.size()) dl.resize(std::max<size_t>({static_cast<size_t>(h) + 1, dl.size() * 2, 1024}), DL_NONE);   // grown: shipped whole
+    if (dl[h] != deadline) {
+        dl[h] = deadline;
+        dirty_dl.push_back(h);
+        dl_heap_.emplace_back(deadline, h);
+        std::push_heap(dl_heap_.begin(), dl_heap_.end(), std::greater<>());
+        dirty = true;
+    }
+    dl_topic_[h].assign(topic, len);
+    if (dl_heap_.size() > 2 * dl_topic_.size() + 4096) {      // mostly stale entries: rebuild from the live deadlines
+        dl_heap_.clear();
+        for (const auto& kv : dl_topic_) dl_heap_.emplace_back(dl[kv.first], kv.first);
+        std::make_heap(dl_heap_.begin(), dl_heap_.end(), std::greater<>());
+    }
+}
+
+void RetainTreeHost::drop_deadline(u32 h) {
+    if (dl_topic_.empty() || !dl_topic_.erase(h)) return;
+    dl[h] = DL_NONE;
+    dirty_dl.push_back(h);
+    dirty = true;
+}
+
+int RetainTreeHost::check_batch(const char* blob, const u32* offsets, const u32* values, const u64* deadlines, u64 n) const {
+    if (!deadlines && dl_topic_.empty()) return PARSE_OK;
+    std::unordered_map<u32, std::pair<bool, std::string_view>> held;   // handle -> (has a deadline, its topic) as the batch goes
+    for (u64 i = 0; i < n; ++i) {
+        const u32 h = values[i];
+        const u64 d = deadlines ? deadlines[i] : 0;
+        if (d && h >= DL_MAX_HANDLE) return SET_HANDLE_RANGE;
+        const std::string_view t(blob + offsets[i], offsets[i + 1] - offsets[i]);
+        auto it = held.find(h);
+        if (it == held.end()) {
+            auto g = dl_topic_.find(h);
+            if (g == dl_topic_.end() && !d) continue;
+            it = held.emplace(h, std::make_pair(g != dl_topic_.end(), g != dl_topic_.end() ? std::string_view(g->second) : std::string_view())).first;
+        }
+        if (it->second.first && it->second.second != t) return SET_CONFLICT;
+        it->second = std::make_pair(d != 0, t);
+    }
+    return PARSE_OK;
+}
+
+u64 RetainTreeHost::set_batch_ttl(const char* blob, const u32* offsets, const u32* values, const u64* deadlines, u64 n) {
+    const u64 ok = set_batch(blob, offsets, values, n);      // (into an empty tree: the parallel build) — clears replaced deadlines
+    std::vector<u32> with;
+    for (u64 i = 0; i < n; ++i) if (deadlines[i]) with.push_back(values[i]);
+    if (with.empty()) return ok;
+    std::sort(with.begin(), with.end());
+    for (u64 i = 0; i < n; ++i) {        // in order, as n set_ttl calls: the last entry of a (topic, handle) the tree holds decides
+        const u32 h = values[i];
+        if (!deadlines[i] && !std::binary_search(with.begin(), with.end(), h)) continue;
+        const char* t = blob + offsets[i];
+        const u32 len = offsets[i + 1] - offsets[i];
+        if (!holds(t, len, h)) continue;
+        if (deadlines[i]) give_deadline(h, t, len, deadlines[i]); else drop_deadline(h);
+    }
+    return ok;
+}
+
+u64 RetainTreeHost::remove_expired(u64 now, u32* out, u64 cap) {
+    u64 n = 0;
+    while (n < cap && !dl_heap_.empty() && dl_heap_.front().first <= now) {
+        std::pop_heap(dl_heap_.begin(), dl_heap_.end(), std::greater<>());
+        const auto [d, h] = dl_heap_.back();
+        dl_heap_.pop_back();
+        auto it = dl_topic_.find(h);
+        if (it == dl_topic_.end() || dl[h] != d) continue;   // re-set or removed since it was queued
+        const std::string topic = it->second;
+        bool had = false; u32 old = 0;
+        remove(topic.data(), static_cast<u32>(topic.size()), &had, &old);    // drops the deadline
+        if (had) out[n++] = old;
+    }
+    return n;
 }
 
 u64 RetainTreeHost::set_batch(const char* blob, const u32* offsets, const u32* values, u64 n) {

@@ -24,6 +24,9 @@
 // Anything involving a literal '+' / '#' level (they shadow wildcard expansion), a hash table more than half full,
 // or too much garbage falls back to a full flatten at the next flush.
 #pragma once
+#include <string>
+#include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "host_trie.h"
@@ -72,10 +75,32 @@ class RetainTreeHost {
   public:
     explicit RetainTreeHost(HostTrie* dict) : dict_(dict) { nodes_.emplace_back(); }
 
-    // RetainTree::insert (retain.rs:221-234): value.replace(v).  Returns ParseStatus; *had_old / *old as remove.
-    int set(const char* topic, u32 len, u32 value, bool* had_old, u32* old);
-    // RetainTree::remove (retain.rs:237-257) with bottom-up pruning.
+    // RetainTree::insert (retain.rs:221-234): value.replace(v).  Returns ParseStatus or SET_CONFLICT; *had_old / *old as
+    // remove.  = set_ttl without a deadline: clears the handle's deadline.
+    int set(const char* topic, u32 len, u32 value, bool* had_old, u32* old) { return set_ttl(topic, len, value, 0, had_old, old); }
+    // RetainTree::remove (retain.rs:237-257) with bottom-up pruning; clears the deadline of the handle it removes.
     int remove(const char* topic, u32 len, bool* had_old, u32* old);
+
+    // ---- deadlines (RetainStorage::set_with_timeout / remove_expired_messages, retain.rs:118-149) ----
+    // A deadline is in ms since the Unix epoch (0 = none) and belongs to a handle; a handle that carries one is stored under
+    // one topic only, whose bytes are kept for the sweep.  A value replaced or removed loses its deadline.  `dl` is the
+    // handle-indexed table the lookup reads (~0 = none); the flush ships it whole when it grew, else its dirty words.
+    static constexpr int SET_CONFLICT = 16;            // status: the handle carries a deadline under another topic (nothing changed)
+    static constexpr int SET_HANDLE_RANGE = 17;        // status: a deadline for a handle >= DL_MAX_HANDLE (nothing changed)
+    static constexpr u32 DL_MAX_HANDLE = 1u << 28;     // the table takes 8 bytes per handle up to the largest one with a deadline
+    static constexpr u64 DL_NONE = ~0ull;
+    int set_ttl(const char* topic, u32 len, u32 value, u64 deadline, bool* had_old, u32* old);
+    // whether n sets with these deadlines (nullptr: none) would store a handle with a deadline under a second topic
+    // (SET_CONFLICT / SET_HANDLE_RANGE) — checked before a batch changes anything; PARSE_OK otherwise
+    int check_batch(const char* blob, const u32* offsets, const u32* values, const u64* deadlines, u64 n) const;
+    // set_batch, then the deadlines of the entries whose handle the tree holds at the end (n set_ttl calls in order)
+    u64 set_batch_ttl(const char* blob, const u32* offsets, const u32* values, const u64* deadlines, u64 n);
+    // removes up to `cap` topics whose handle's deadline is <= now, earliest first; their handles go to out[]
+    u64 remove_expired(u64 now, u32* out, u64 cap);
+    u32 dl_lookup_size() const { return dl_topic_.empty() ? 0u : static_cast<u32>(dl.size()); }   // 0: the lookup ignores deadlines
+    std::vector<u64> dl;
+    std::vector<u32> dirty_dl;
+    bool full_dl = true;
     // n sets (start-up / restore: every retained message re-enters the tree, rmqtt-retainer/src/retainer.rs load path).
     // Returns the number of valid topics.  Into an EMPTY tree the host tree and its device image are built together, level
     // by level, on all host threads (set_batch_build); otherwise one by one.
@@ -91,7 +116,7 @@ class RetainTreeHost {
     bool dirty = true;          // something to ship (whole arrays or patches)
     bool full = true;           // the arrays were rebuilt: ship them whole
     void prepare_flush();       // makes the arrays below current (flattens if in-place maintenance gave up)
-    void shipped() { dirty = false; full = false; dirty_kids.clear(); dirty_edges.clear(); dirty_vals.clear(); }
+    void shipped() { dirty = false; full = false; dirty_kids.clear(); dirty_edges.clear(); dirty_vals.clear(); dirty_dl.clear(); full_dl = false; }
     void flatten();                                     // host tree -> device-layout arrays below
     std::vector<RNode, HugeAlloc<RNode>> rnodes;        // host bookkeeping, one per device node (not shipped)
     std::vector<RKid, HugeAlloc<RKid>> rkids;
@@ -127,6 +152,12 @@ class RetainTreeHost {
     u64 set_batch_build(const char* blob, const u32* offsets, const u32* values, u64 n, unsigned threads);
     int parse(const char* s, u32 len, bool create, std::vector<u32>& toks);
     u32 child_of(u32 node, u32 token) const;
+    int put(const char* topic, u32 len, u32 value, bool* had_old, u32* old);
+    bool holds(const char* topic, u32 len, u32 value);           // the topic's value is `value`
+    void give_deadline(u32 h, const char* topic, u32 len, u64 deadline);
+    void drop_deadline(u32 h);
+    std::unordered_map<u32, std::string> dl_topic_;              // handle -> the topic it carries its deadline under
+    std::vector<std::pair<u64, u32>> dl_heap_;                   // (deadline, handle), min-heap; stale once the handle's deadline changed
     HostTrie* dict_;
     BigVec<HN> nodes_;
     std::vector<u32> free_;

@@ -187,12 +187,23 @@ class Engine:
         return self.match_topics([topic]).sorted_list(0)
 
     # ---- retained-message tree: RetainTree insert / remove / matches (rmqtt/src/retain.rs) ------------------
-    def retain_set(self, topic, value: int):
-        """Returns the replaced value or None."""
+    def retain_set(self, topic, value: int, deadline_ms: int | None = None):
+        """Returns the replaced value or None.  deadline_ms (ms since the Unix epoch; None or 0: none) expires the value
+        at that time (gm_retain_set_ttl); setting a handle without one clears its deadline."""
         b = _b(topic)
         had, old = C.c_int32(0), C.c_uint32(0)
-        self._check(self._lib.gm_retain_set(self._h, b, len(b), value, C.byref(had), C.byref(old)))
+        if deadline_ms is None:
+            self._check(self._lib.gm_retain_set(self._h, b, len(b), value, C.byref(had), C.byref(old)))
+        else:
+            self._check(self._lib.gm_retain_set_ttl(self._h, b, len(b), value, int(deadline_ms), C.byref(had), C.byref(old)))
         return int(old.value) if had.value else None
+
+    def retain_remove_expired(self, now_ms: int, cap: int) -> np.ndarray:
+        """remove_expired_messages: removes up to `cap` expired topics (earliest deadline first) -> their handles."""
+        out = np.empty(max(int(cap), 1), dtype=np.uint32)
+        n = C.c_uint64(0)
+        self._check(self._lib.gm_retain_remove_expired(self._h, int(now_ms), _vp(out), int(cap), C.byref(n)))
+        return out[:int(n.value)].copy()
 
     def retain_remove(self, topic):
         b = _b(topic)
@@ -209,12 +220,19 @@ class Engine:
         self._check(self._lib.gm_retain_remove_batch(self._h, _vp(blob), _vp(offs), n, _vp(old), C.byref(cnt)))
         return old, int(cnt.value)
 
-    def retain_bulk_load(self, blob: np.ndarray, offs: np.ndarray, values: np.ndarray) -> int:
+    def retain_bulk_load(self, blob: np.ndarray, offs: np.ndarray, values: np.ndarray, deadlines_ms: np.ndarray | None = None) -> int:
+        """deadlines_ms (uint64[n], 0 = none): gm_retain_bulk_load_ttl."""
         n_set = C.c_uint64(0)
-        self._check(self._lib.gm_retain_bulk_load(self._h, _vp(blob), _vp(offs), _vp(values), len(values), C.byref(n_set)))
+        if deadlines_ms is None:
+            self._check(self._lib.gm_retain_bulk_load(self._h, _vp(blob), _vp(offs), _vp(values), len(values), C.byref(n_set)))
+        else:
+            dl = np.ascontiguousarray(deadlines_ms, dtype=np.uint64)
+            assert len(dl) == len(values)
+            self._check(self._lib.gm_retain_bulk_load_ttl(self._h, _vp(blob), _vp(offs), _vp(values), _vp(dl), len(values), C.byref(n_set)))
         return int(n_set.value)
 
-    def retain_match_batch(self, blob: np.ndarray, offs: np.ndarray, cap_ids: int | None = None) -> MatchResult:
+    def retain_match_batch(self, blob: np.ndarray, offs: np.ndarray, cap_ids: int | None = None, now_ms: int | None = None) -> MatchResult:
+        """now_ms (ms since the Unix epoch): evaluate deadlines at that time (gm_retain_match_batch_at); None: the wall clock."""
         n = len(offs) - 1
         spans = np.zeros((n, 2), dtype=np.uint32)
         status = np.zeros(n, dtype=np.int32)
@@ -222,16 +240,19 @@ class Engine:
         while True:
             ids = np.empty(cap, dtype=np.uint32)
             needed = C.c_uint64(0)
-            rc = self._lib.gm_retain_match_batch(self._h, _vp(blob), _vp(offs), n, _vp(spans), _vp(ids), cap, C.byref(needed), _vp(status))
+            if now_ms is None:
+                rc = self._lib.gm_retain_match_batch(self._h, _vp(blob), _vp(offs), n, _vp(spans), _vp(ids), cap, C.byref(needed), _vp(status))
+            else:
+                rc = self._lib.gm_retain_match_batch_at(self._h, int(now_ms), _vp(blob), _vp(offs), n, _vp(spans), _vp(ids), cap, C.byref(needed), _vp(status))
             if rc == N.GM_ERR_CAPACITY and cap_ids is None:
                 cap = int(needed.value)
                 continue
             self._check(rc)
             return MatchResult(spans, ids[:int(needed.value)], status, int(needed.value))
 
-    def retain_matches(self, filt):
+    def retain_matches(self, filt, now_ms: int | None = None):
         blob, offs = pack([filt])
-        return self.retain_match_batch(blob, offs).sorted_list(0)
+        return self.retain_match_batch(blob, offs, now_ms=now_ms).sorted_list(0)
 
     def retain_match_batch_device(self, d_blob, d_offs, d_spans, d_ids, d_status, stream: int) -> int:
         n = d_offs.numel() - 1
