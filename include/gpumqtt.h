@@ -233,6 +233,72 @@ int32_t gm_retain_match_batch_at(gm_engine* e, uint64_t now_ms, const char* filt
  * their handles, so that the caller can drop the payloads.  Loop while *n_removed == cap.  The cost grows with the number
  * removed (a deadline-ordered queue), not with the size of the tree.                                                      */
 int32_t gm_retain_remove_expired(gm_engine* e, uint64_t now_ms, uint32_t* out_values, uint64_t cap, uint64_t* n_removed);
+/* gm_retain_match_batch_device at `now_ms` instead of the wall clock. */
+int32_t gm_retain_match_batch_device_at(gm_engine* e, uint64_t now_ms, const void* d_filters_blob, uint64_t blob_bytes,
+                                        const uint32_t* d_filter_offsets, uint64_t n, gm_span* d_out_spans, uint32_t* d_out_ids,
+                                        uint64_t cap_ids, uint64_t* needed, int32_t* d_status, void* stream);
+
+/* ---- message store: rmqtt-message-storage's RAM backend (rmqtt-plugins/rmqtt-message-storage/src/ram.rs) — the messages kept
+ *      for offline and late subscribers, looked up on every SUBSCRIBE, with the per-client "already forwarded" marks
+ *      (ram.rs:120 `forwardeds`) kept, checked and set on the device.  Payloads and `from` stay with the caller, by handle.
+ *   - The store OWNS its engine's retained tree: a broker that also runs the retainer gives the store an engine of its own.
+ *     A message is kept under the key  topic + "/" + decimal(handle)  (ram.rs:266-267 pushes the MsgID as a level), so a caller
+ *     whose MsgIDs are the handles gets the reference's results exactly, including `a/5/#` returning message 5 published to `a`.
+ *     A key has one level more than its topic and a query one more than its filter: give the store's engine a max_levels one
+ *     above the broker's limit.
+ *   - Handles are below GM_RETAIN_TTL_MAX_HANDLE (every stored message has an expiry, rmqtt/src/session.rs:1810-1815).  A handle
+ *     is stored once; it may be stored again after the sweep removed it, and then starts with no marks.
+ *   - Keys are chosen by the caller and are below 2^31.  A client key names a ClientId.  A share key names a (topic filter,
+ *     shared group) pair: equal pairs must carry equal keys (rmqtt_b200/msgstore.py interns both).
+ *   - A mark is (client key, share key or GM_MSGSTORE_NO_SHARE).  Marks given to store are applied as BTreeMap::insert is
+ *     (ram.rs:247-256): the last entry for a client wins.
+ * gm_msgstore_get_batch is ram.rs `get` (:303-367) for a batch of SUBSCRIBE filters, with the same span, capacity and status
+ * protocol as gm_retain_match_batch_at.  Query i = (filter i, client_keys[i], share_keys[i]):
+ *   - the filter gets a '+' level appended unless its last level is '#', and is matched against the stored keys;
+ *   - an expired message (expiry_time_at < now_ms, rmqtt/src/types.rs:1883-1885) is neither returned nor marked;
+ *   - a message is returned iff it was not already forwarded to the query: its client key is not marked on it and, for a shared
+ *     query, its share key is not marked on it.  The marks that count are those given to store, those of earlier calls and
+ *     those of the EARLIER queries of the same batch: a batch returns what its queries return run one at a time in batch order.
+ *     Within a query, handles are unordered;
+ *   - a returned message is marked with the query's client key, and with its share key when the query is shared.
+ * A call that fails marks nothing (GM_ERR_CAPACITY, GM_ERR_TOO_LARGE, a CUDA error); a retry with cap = *needed returns the
+ * same lists and marks them.  An invalid filter yields an empty list and marks nothing.
+ * gm_msgstore_remove_expired is remove_expired_messages (ram.rs:143-191): it removes the messages with expiry_time_at <= now_ms,
+ * earliest first, at most `cap` of them, and returns their handles; their marks go with them.  A caller enforcing
+ * cache_max_count / cache_capacity (ram.rs:152-171) evicts the k earliest-expiring messages with now_ms = UINT64_MAX - 1 and
+ * cap = k.                                                                                                                   */
+typedef struct gm_msgstore gm_msgstore;
+#define GM_MSGSTORE_NO_SHARE 0xFFFFFFFFu
+typedef struct gm_msgstore_config {
+    uint32_t struct_size;         /* = sizeof(gm_msgstore_config) */
+    uint32_t initial_mark_slots;  /* slots of the mark set at creation, a power of two >= 64 (0 = default 65536); it grows by itself */
+} gm_msgstore_config;
+typedef struct gm_msgstore_stats {
+    uint64_t messages;            /* stored and not yet swept */
+    uint64_t marks;               /* entries of the device mark set (a client key or a share key on a message) */
+    uint64_t pending_marks;       /* entries given to store and not yet on the device (inserted before the next lookup) */
+    uint64_t mark_slots;          /* slots of the device mark set (8 bytes each, load <= 1/2) */
+    uint64_t rehashes;            /* times the mark set grew */
+    uint64_t purges;              /* rebuilds that dropped the marks of swept messages */
+    uint64_t retired;             /* swept handles whose marks are still in the set (dropped by the next rebuild) */
+} gm_msgstore_stats;
+int32_t gm_msgstore_create(gm_engine* e, const gm_msgstore_config* cfg, gm_msgstore** out);   /* the store uses, but does not own, the engine */
+void gm_msgstore_destroy(gm_msgstore* ms);
+/* _set (ram.rs:259-300): keep message `handle` published to `topic` until expiry_time_at_ms (< UINT64_MAX), marked as forwarded
+ * to the n_marks (client_keys[i], share_keys[i]) it was delivered to (share_keys may be NULL: none shared).                      */
+int32_t gm_msgstore_store(gm_msgstore* ms, const char* topic, uint32_t len, uint32_t handle, uint64_t expiry_time_at_ms,
+                          const uint32_t* client_keys, const uint32_t* share_keys, uint32_t n_marks);
+/* n gm_msgstore_store calls at once, through the engine's bulk load (restore): message i's marks are
+ * [mark_offsets[i], mark_offsets[i+1]) of client_keys / share_keys (mark_offsets NULL: no marks).  Nothing changes when one
+ * message is refused.                                                                                                           */
+int32_t gm_msgstore_store_batch(gm_msgstore* ms, const char* blob, const uint32_t* offsets /* n+1 */, const uint32_t* handles,
+                                const uint64_t* expiry_time_at_ms, uint64_t n, const uint32_t* mark_offsets /* n+1 */,
+                                const uint32_t* client_keys, const uint32_t* share_keys);
+int32_t gm_msgstore_get_batch(gm_msgstore* ms, uint64_t now_ms, const char* filters_blob, const uint32_t* filter_offsets, uint64_t n,
+                              const uint32_t* client_keys, const uint32_t* share_keys, gm_span* out_spans, uint32_t* out_handles,
+                              uint64_t cap, uint64_t* needed, int32_t* status);
+int32_t gm_msgstore_remove_expired(gm_msgstore* ms, uint64_t now_ms, uint32_t* out_handles, uint64_t cap, uint64_t* n_removed);
+int32_t gm_msgstore_stats_get(gm_msgstore* ms, gm_msgstore_stats* out);
 
 /* ---- GpuRouter: DefaultRouter's Router-level semantics above the engine (rmqtt/src/router.rs:109-115, 162-248,
  *      417-479; rmqtt/src/types.rs:470-508).  This is what a Rust `GpuRouter` keeps on the host (INTEGRATION.md);

@@ -358,3 +358,52 @@ extern "C" {
     pub fn gm_device_numa_node(device: i32) -> i32;
     pub fn gm_bind_thread_near_device(device: i32) -> i32;
 }
+
+// ---- message store (rmqtt-message-storage's RAM backend with the forwarded marks on the device) ----
+#[repr(C)]
+pub struct gm_msgstore {
+    _private: [u8; 0],
+}
+
+pub const GM_MSGSTORE_NO_SHARE: u32 = 0xFFFF_FFFF;
+
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct gm_msgstore_config {
+    pub struct_size: u32,
+    pub initial_mark_slots: u32,
+}
+
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct gm_msgstore_stats {
+    pub messages: u64,
+    pub marks: u64,
+    pub pending_marks: u64,
+    pub mark_slots: u64,
+    pub rehashes: u64,
+    pub purges: u64,
+    pub retired: u64,
+}
+
+extern "C" {
+    /// gm_retain_match_batch_device at `now_ms`.
+    pub fn gm_retain_match_batch_device_at(e: *mut gm_engine, now_ms: u64, d_filters_blob: *const c_void, blob_bytes: u64, d_filter_offsets: *const u32,
+                                           n: u64, d_out_spans: *mut gm_span, d_out_ids: *mut u32, cap_ids: u64, needed: *mut u64, d_status: *mut i32,
+                                           stream: *mut c_void) -> i32;
+    /// The store owns its engine's retained tree: give it an engine of its own, with max_levels one above the broker's.
+    pub fn gm_msgstore_create(e: *mut gm_engine, cfg: *const gm_msgstore_config, out: *mut *mut gm_msgstore) -> i32;
+    pub fn gm_msgstore_destroy(ms: *mut gm_msgstore);
+    /// _set: the message is kept under topic/<handle> until expiry_time_at_ms, marked as forwarded to (client_keys[i], share_keys[i]).
+    pub fn gm_msgstore_store(ms: *mut gm_msgstore, topic: *const u8, len: u32, handle: u32, expiry_time_at_ms: u64, client_keys: *const u32,
+                             share_keys: *const u32, n_marks: u32) -> i32;
+    pub fn gm_msgstore_store_batch(ms: *mut gm_msgstore, blob: *const u8, offsets: *const u32, handles: *const u32, expiry_time_at_ms: *const u64, n: u64,
+                                   mark_offsets: *const u32, client_keys: *const u32, share_keys: *const u32) -> i32;
+    /// get for a batch of SUBSCRIBE filters, in batch order; returned messages are marked as forwarded to their query.
+    pub fn gm_msgstore_get_batch(ms: *mut gm_msgstore, now_ms: u64, filters_blob: *const u8, filter_offsets: *const u32, n: u64, client_keys: *const u32,
+                                 share_keys: *const u32, out_spans: *mut gm_span, out_handles: *mut u32, cap: u64, needed: *mut u64,
+                                 status: *mut i32) -> i32;
+    /// remove_expired_messages: expiry_time_at <= now_ms, earliest first; now_ms = u64::MAX - 1 evicts the `cap` earliest-expiring.
+    pub fn gm_msgstore_remove_expired(ms: *mut gm_msgstore, now_ms: u64, out_handles: *mut u32, cap: u64, n_removed: *mut u64) -> i32;
+    pub fn gm_msgstore_stats_get(ms: *mut gm_msgstore, out: *mut gm_msgstore_stats) -> i32;
+}

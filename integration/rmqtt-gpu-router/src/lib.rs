@@ -482,3 +482,83 @@ impl RetainStorage for GpuRetainer {
     async fn count(&self) -> isize { self.slots.len() as isize }
     async fn max(&self) -> isize { self.slots.len() as isize }
 }
+
+// ---- message store --------------------------------------------------------------------------------------------------
+/// rmqtt-message-storage's `MessageManager` with `get`'s forwarded checks and marks on the device (gm_msgstore_*).
+/// The store owns the retained tree of its engine: it gets an engine of its own, with max_levels one above the listener's.
+pub mod msgstore {
+    #![allow(unsafe_code)]
+    use super::engine::Engine;
+    use dashmap::DashMap;
+    use gpumqtt_sys as sys;
+    use rmqtt::{timestamp_millis, From, MsgID, Publish, Result, SharedGroup, SubClientIds};
+    use std::time::Duration;
+
+    pub struct GpuMessageManager {
+        engine: Engine,
+        store: *mut sys::gm_msgstore,
+        msgs: DashMap<MsgID, (From, Publish)>,               // payloads and senders stay on the host, by message id
+        clients: DashMap<String, u32>,                       // ClientId -> client key
+        shares: DashMap<(String, String), u32>,              // (topic filter, group) -> share key: equal pairs, equal keys
+    }
+    unsafe impl Send for GpuMessageManager {}
+    unsafe impl Sync for GpuMessageManager {}               // gm_msgstore calls are serialised inside the library
+
+    impl GpuMessageManager {
+        pub fn new(engine: Engine) -> anyhow::Result<Self> {
+            let mut store = std::ptr::null_mut();
+            let rc = unsafe { sys::gm_msgstore_create(engine.0, std::ptr::null(), &mut store) };
+            anyhow::ensure!(rc == sys::GM_OK, "gm_msgstore_create: {rc}");
+            Ok(Self { engine, store, msgs: DashMap::default(), clients: DashMap::default(), shares: DashMap::default() })
+        }
+        fn client_key(&self, c: &str) -> u32 { let n = self.clients.len() as u32; *self.clients.entry(c.to_owned()).or_insert(n) }
+        fn share_key(&self, f: &str, g: &str) -> u32 { let n = self.shares.len() as u32; *self.shares.entry((f.to_owned(), g.to_owned())).or_insert(n) }
+
+        /// ram.rs:259-300 (`_set`): kept under topic/<msg_id> until now + expiry_interval, marked as forwarded to sub_client_ids
+        pub fn store(&self, msg_id: MsgID, from: From, p: Publish, expiry_interval: Duration, sub_client_ids: SubClientIds) -> Result<()> {
+            let at = timestamp_millis() as u64 + expiry_interval.as_millis() as u64;
+            let (cl, sh): (Vec<u32>, Vec<u32>) = sub_client_ids.unwrap_or_default().iter()
+                .map(|(c, s)| (self.client_key(c), s.as_ref().map(|(f, g)| self.share_key(f, g)).unwrap_or(sys::GM_MSGSTORE_NO_SHARE)))
+                .unzip();
+            let topic = p.topic.clone();
+            self.msgs.insert(msg_id, (from, p));
+            let rc = unsafe { sys::gm_msgstore_store(self.store, topic.as_ptr(), topic.len() as u32, msg_id as u32, at, cl.as_ptr(), sh.as_ptr(), cl.len() as u32) };
+            if rc != sys::GM_OK { self.msgs.remove(&msg_id); anyhow::bail!("gm_msgstore_store: {rc}") }
+            Ok(())
+        }
+
+        /// ram.rs:303-367 (`get`): the device drops what was forwarded or expired and marks what it returns
+        pub fn get(&self, client_id: &str, topic_filter: &str, group: Option<&SharedGroup>) -> Result<Vec<(MsgID, From, Publish)>> {
+            let cl = [self.client_key(client_id)];
+            let sh = [group.map(|g| self.share_key(topic_filter, g)).unwrap_or(sys::GM_MSGSTORE_NO_SHARE)];
+            let offs = [0u32, topic_filter.len() as u32];
+            let (mut span, mut status, mut needed) = (sys::gm_span { off: 0, cnt: 0 }, 0i32, 0u64);
+            let mut out = vec![0u32; 256];
+            loop {
+                let rc = unsafe { sys::gm_msgstore_get_batch(self.store, timestamp_millis() as u64, topic_filter.as_ptr(), offs.as_ptr(), 1, cl.as_ptr(),
+                                                             sh.as_ptr(), &mut span, out.as_mut_ptr(), out.len() as u64, &mut needed, &mut status) };
+                if rc == sys::GM_ERR_CAPACITY { out.resize(needed as usize, 0); continue }   // nothing was marked: ask again
+                anyhow::ensure!(rc == sys::GM_OK, "gm_msgstore_get_batch: {rc}");
+                anyhow::ensure!(status == sys::GM_OK, "invalid topic filter");
+                break;
+            }
+            Ok(out[span.off as usize..(span.off + span.cnt) as usize].iter()
+                .filter_map(|h| self.msgs.get(&(*h as MsgID)).map(|m| (*h as MsgID, m.0.clone(), m.1.clone()))).collect())
+        }
+
+        /// ram.rs:143-191: expiry_time_at <= now, earliest first; `evict` (cache_max_count / cache_capacity) takes the k earliest-expiring
+        pub fn remove_expired_messages(&self, evict: Option<usize>) -> usize {
+            const CAP: usize = 65_536;
+            let (now, cap) = match evict { Some(k) => (u64::MAX - 1, k), None => (timestamp_millis() as u64, CAP) };
+            let mut out = vec![0u32; cap.max(1)];
+            let mut n = 0u64;
+            if unsafe { sys::gm_msgstore_remove_expired(self.store, now, out.as_mut_ptr(), cap as u64, &mut n) } != sys::GM_OK { return 0 }
+            for h in &out[..n as usize] { self.msgs.remove(&(*h as MsgID)); }
+            n as usize
+        }
+    }
+
+    impl Drop for GpuMessageManager {
+        fn drop(&mut self) { unsafe { sys::gm_msgstore_destroy(self.store) } }
+    }
+}

@@ -35,7 +35,7 @@ def _newer(target: Path, sources) -> bool:
 
 
 def build_engine(force: bool = False, verbose: bool = False) -> Path:
-    srcs = [CSRC / "engine.cu", CSRC / "host_trie.cpp", CSRC / "retain_tree.cpp", CSRC / "router_host.cpp", CSRC / "batcher.cpp", CSRC / "retain_batcher.cpp"]
+    srcs = [CSRC / "engine.cu", CSRC / "host_trie.cpp", CSRC / "retain_tree.cpp", CSRC / "router_host.cpp", CSRC / "batcher.cpp", CSRC / "retain_batcher.cpp", CSRC / "msgstore.cu"]
     deps = srcs + sorted(CSRC.glob("*.h")) + sorted(CSRC.glob("*.cuh")) + [PKG.parent / "include" / "gpumqtt.h"]
     if force or _newer(LIB, deps):
         cmd = [_nvcc(), *NVCC_FLAGS, "-o", str(LIB), *map(str, srcs)]

@@ -106,6 +106,20 @@ class GmGatherView(C.Structure):
                 ("slab_topics", C.c_uint64), ("slab_ids", C.c_uint64), ("world", C.c_uint32), ("rank", C.c_uint32)]
 
 
+GM_MSGSTORE_NO_SHARE = 0xFFFFFFFF
+
+
+class GmMsgstoreConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("initial_mark_slots", C.c_uint32)]
+
+
+class GmMsgstoreStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("messages", "marks", "pending_marks", "mark_slots", "rehashes", "purges", "retired")]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
 class GmValues(C.Structure):
     _fields_ = [("values", C.c_void_p), ("n_values", C.c_uint64), ("ranges", C.c_void_p), ("n_ranges", C.c_uint64), ("epoch", C.c_uint64)]
 
@@ -167,6 +181,14 @@ SIGNATURES = {
     "gm_retain_bulk_load_ttl": (_i32, [_vp, _vp, _vp, _vp, _vp, _u64, _P(_u64)]),
     "gm_retain_match_batch_at": (_i32, [_vp, _u64, _vp, _vp, _u64, _vp, _vp, _u64, _P(_u64), _vp]),
     "gm_retain_remove_expired": (_i32, [_vp, _u64, _vp, _u64, _P(_u64)]),
+    "gm_retain_match_batch_device_at": (_i32, [_vp, _u64, _vp, _u64, _vp, _u64, _vp, _vp, _u64, _P(_u64), _vp, _vp]),
+    "gm_msgstore_create": (_i32, [_vp, _P(GmMsgstoreConfig), _P(_vp)]),
+    "gm_msgstore_destroy": (None, [_vp]),
+    "gm_msgstore_store": (_i32, [_vp, _cp, _u32, _u32, _u64, _vp, _vp, _u32]),
+    "gm_msgstore_store_batch": (_i32, [_vp, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp]),
+    "gm_msgstore_get_batch": (_i32, [_vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _u64, _P(_u64), _vp]),
+    "gm_msgstore_remove_expired": (_i32, [_vp, _u64, _vp, _u64, _P(_u64)]),
+    "gm_msgstore_stats_get": (_i32, [_vp, _P(GmMsgstoreStats)]),
     "gmr_create": (_i32, [_vp, _P(_vp)]),
     "gmr_destroy": (None, [_vp]),
     "gmr_add": (_i32, [_vp, _cp, _u32, _P(GmId), _P(GmSubOpts)]),

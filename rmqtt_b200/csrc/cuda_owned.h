@@ -94,6 +94,7 @@ using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
 using Event = Owned<cudaEvent_t, cudaEventDestroy>;
 using GraphExec = Owned<cudaGraphExec_t, cudaGraphExecDestroy>;
 
+int engine_device(gm_engine* e);       // the engine's CUDA device, -1 for a host-only engine (engine.cu)
 void nccl_comm_destroy(ncclComm* c);   // ncclCommDestroy through NcclApi, which binds libnccl at run time (engine.cu)
 using NcclComm = Owned<ncclComm*, nccl_comm_destroy>;
 

@@ -1122,7 +1122,11 @@ int32_t gm_retain_bulk_load_ttl(gm_engine* e, const char* blob, const uint32_t* 
 
 int32_t gm_retain_match_batch_device(gm_engine* e, const void* d_blob, uint64_t blob_bytes, const uint32_t* d_offs, uint64_t n,
                                      gm_span* d_spans, uint32_t* d_ids, uint64_t cap_ids, uint64_t* needed, int32_t* d_status, void* stream) {
-    const u64 now_ms = wall_ms();
+    return gm_retain_match_batch_device_at(e, wall_ms(), d_blob, blob_bytes, d_offs, n, d_spans, d_ids, cap_ids, needed, d_status, stream);
+}
+
+int32_t gm_retain_match_batch_device_at(gm_engine* e, uint64_t now_ms, const void* d_blob, uint64_t blob_bytes, const uint32_t* d_offs, uint64_t n,
+                                        gm_span* d_spans, uint32_t* d_ids, uint64_t cap_ids, uint64_t* needed, int32_t* d_status, void* stream) {
     if (!e || (n && (!d_offs || !d_spans || !d_status))) return GM_ERR_INVALID_ARG;
     if (needed) *needed = 0;
     if (n == 0) return GM_OK;
@@ -1185,6 +1189,13 @@ int32_t gm_retain_match_batch_at(gm_engine* e, uint64_t now_ms, const char* blob
     }
     return GM_OK;
 }
+
+}  // extern "C"
+
+// the engine's CUDA device, -1 for a host-only engine (the message store, msgstore.cu, runs its kernels there)
+int gm::engine_device(gm_engine* e) { return (e->flags & GM_FLAG_HOST_ONLY) ? -1 : e->device; }
+
+extern "C" {
 
 // ---- GpuRouter (router_host.cpp) ------------------------------------------------------------------------
 struct gm_router { GpuRouter impl; explicit gm_router(gm_engine* e) : impl(e) {} };
