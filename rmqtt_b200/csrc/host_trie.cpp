@@ -1060,6 +1060,7 @@ void HostTrie::compact(const std::vector<u32>* keep, std::vector<u32>* remap) {
             const u32 neu = fresh.intern(tok_str[old].data(), static_cast<u32>(tok_str[old].size()), true);
             if (remap) (*remap)[old] = neu;
         }
+    fresh.values_epoch = values_epoch + 1;           // `values` was rebuilt: descriptors of an earlier epoch are stale (gm_values)
     *this = std::move(fresh);
 }
 

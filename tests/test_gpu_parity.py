@@ -376,42 +376,6 @@ def test_capacity_error_reports_needed_across_pipeline_chunks():
     assert (i1 == i2).all()
 
 
-def test_thread_safety_concurrent_matches_and_mutations():
-    import threading
-    cfg = wl.C2.scaled(n_subs=30_000, n_topics=20_000)
-    sb, so, sv = wl.gen_subs(cfg)
-    tb, to = wl.gen_topics(cfg)
-    eng = Engine()
-    eng.bulk_load(sb, so, sv)
-    base = eng.match_batch(tb, to).counts()
-    errors = []
-
-    def reader():
-        try:
-            for _ in range(6):
-                c = eng.match_batch(tb, to).counts()
-                # the writer only ever adds/removes the filter "zz/never/#", which matches no topic of the batch
-                assert (c == base).all()
-        except Exception as ex:          # noqa: BLE001
-            errors.append(ex)
-
-    def writer():
-        try:
-            for i in range(200):
-                eng.add("zz/never/#", i)
-                eng.remove("zz/never/#", i)
-        except Exception as ex:          # noqa: BLE001
-            errors.append(ex)
-
-    ths = [threading.Thread(target=reader) for _ in range(3)] + [threading.Thread(target=writer)]
-    for t in ths:
-        t.start()
-    for t in ths:
-        t.join()
-    assert not errors, errors
-    assert eng.matches("zz/never/x") == []
-
-
 def test_compact_on_device_keeps_parity():
     rng = random.Random(77)
     eng, tree = Engine(), orc.TopicTree()
